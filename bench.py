@@ -1,16 +1,19 @@
 """Benchmark of the denoising hot path (BASELINE.json metric: denoise-steps/sec, 16 f x 512^2 SD-1.5 UNet3D).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--dump-outputs DIR]
 
 One "step" = one loop body of the reference pipeline (pipelines/pipeline_videoswap.py:556-587): CFG batch
 duplication, AnimateDiffUNet3DModel forward on [2,4,16,64,64], CFG combine, DDIM update.  Workload = BASELINE config
-"16-frame 512x512 ... 1xB200 fp16" with ED-LoRA per-layer embeddings and adapter residuals active (superset of
+"16-frame 512x512 ... 1xH100 fp16" with ED-LoRA per-layer embeddings and adapter residuals active (superset of
 configs[1] and configs[2]); synthetic inputs, seeded random weights of the real architecture (no checkpoints offline).
 N > 1 (default --mode shard): one process per GPU (torchrun), ONE video split over the ranks -- strong scaling: N = 2 the two
 CFG halves (one all-gather of the noise predictions per step), N = 4 / 8 CFG x 2 / 4 frame shards (GroupNorm-statistics
 all-reduces + frames<->pixels all-to-all around the motion modules, NCCL over NVLink, captured in the CUDA graph);
 `value` = steps of that one video per second.  --mode replicas: one video per rank (weak scaling, no data-path
 collective).  Barrier + device timing, max over ranks.
+--dump-outputs DIR writes the latents the timed CUDA-graph path returned from its last step as DIR/latents.npy (fp32;
+with --gpus N in shard mode the frame shards of all ranks are gathered, so the file holds the whole video);
+weights and inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -36,19 +39,15 @@ CATS = ["gemm", "conv3x3", "attention", "temporal_attention", "groupnorm", "laye
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return {"tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0)), "tflops_burst": d.get("bf16_tflops", 1590.0),
-                "gbs": d.get("hbm_gbs", 6650.0), "source": "MEASURED_PEAKS.json (sustained bf16 cuBLAS / copy)"}
-    return {"tflops": 1400.0, "tflops_burst": 1590.0, "gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # data-sheet figures (dense FP16 tensor rate, HBM3 bandwidth) of a 700 W card; a card with a lower power limit
+    # reaches less, so frac_of_peak is a lower bound of the share of what that card can do
+    return {"tflops": 989.0, "gbs": 3350.0, "source": "NVIDIA H100 SXM data sheet (dense FP16, HBM3; 700 W)"}
 
 
 class ClockSampler:
     """Samples nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
-        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+        "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, index: int):
         self.rows, self.proc, self.index = [], None, index
@@ -69,11 +68,14 @@ class ClockSampler:
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
+        self.proc.wait()
         sm = sorted(float(r[0]) for r in self.rows if r and r[0].replace(".", "").isdigit())
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(len(r) > 3 + i and r[3 + i] == "Active" for r in self.rows)]
+        pl = [float(r[7]) for r in self.rows if len(r) > 7 and r[7].replace(".", "").isdigit()]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
+                "power_limit_w": pl[0] if pl else None,
                 "samples": len(self.rows)}
 
 
@@ -103,8 +105,7 @@ def cpu_oracle_sample(frames=2, latent=LATENT, reps_budget_s=15.0, warmup=1, max
     import torch
     from oracle import unet3d_oracle as O
     from videoswap_b200 import UNetConfig, seeded_state_dict, unet_param_shapes
-    # measured on the 128-core GPU box (tools/cpu_thread_sweep.py): 16 threads 5.8 s, 32: 6.0 s, 64: 8.9 s, 128: 138 s per
-    # sample -- the sample's tensors are too small for more threads, so the baseline uses the fastest setting
+    # the sample's tensors are too small for many threads: beyond 16, more threads make the sample slower
     torch.set_num_threads(min(os.cpu_count() or 1, 16))
     sd = seeded_state_dict(unet_param_shapes(UNetConfig()), seed=0)
     x = torch.randn(1, 4, frames, latent, latent)
@@ -170,7 +171,7 @@ def library_baseline(sd16, dev, lat0, embeds, residuals, ts, native_out, steps=5
 
 def run_reference(args, rank, world):
     """--impl reference: the reference's CPU path.  The reference is pure Python on diffusers (not installable offline)
-    and /root/reference does not travel to the GPU box, so this times oracle/ (the pinned CPU restatement) on the host
+    and the reference is not available where the benchmark runs, so this times oracle/ (the pinned CPU restatement) on the host
     cores; rank 0 only."""
     if rank != 0:
         return
@@ -206,7 +207,9 @@ def main():
                     help="multi-GPU scheme: ONE video split over the ranks (CFG halves x frame shards; strong scaling, "
                          "default) or independent videos per rank (weak scaling)")
     ap.add_argument("--option", action="append", default=[], help="kernel A/B switch name=value (vs_set_option)")
-    ap.add_argument("--tag", default="", help="suffix of the per-shape profile CSV")
+    ap.add_argument("--profile-csv", default=None, help="write the per-shape kernel profile of the eager pass to this CSV")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the latents of the last timed step as DIR/latents.npy (fp32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -295,9 +298,8 @@ def main():
         a, b, c = C.c_double(), C.c_double(), C.c_longlong()
         _lib.call("vs_profile_collect", ci, C.byref(a), C.byref(b), C.byref(c))
         prof[name] = {"ms_per_step": a.value / K, "work_per_step": b.value / K, "launches_per_step": c.value / K}
-    if rank == 0:
-        os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-        lib.vs_profile_dump(os.path.join(ROOT, "gpurun_out", f"profile_shapes_n{world}{args.tag}.csv").encode())
+    if rank == 0 and args.profile_csv:
+        _lib.call("vs_profile_dump", os.path.abspath(args.profile_csv).encode())
     lib.vs_profile_reset()
     finite = bool(torch.isfinite(lat).all().item())
     ms_eager = ms
@@ -325,6 +327,17 @@ def main():
             dist.barrier()
             ms = t.item()
         finite = finite and bool(torch.isfinite(lat).all().item())
+    timed_out = None                       # what the timed path returned from its last step (the graph reuses its buffers)
+    if args.dump_outputs:
+        if sharded:                        # each rank holds its frame shard: gather the whole video (ranks of the two CFG
+            parts = [torch.empty_like(lat) for _ in range(world)]     # halves hold the same frames; one copy per shard)
+            dist.all_gather(parts, lat.contiguous())
+            first = {}
+            for r in range(world):
+                first.setdefault(dist_util.make_plan(world, r, cfg=True).frame_shard, r)
+            timed_out = torch.cat([parts[first[s]] for s in sorted(first)], dim=2).float().cpu()
+        else:
+            timed_out = lat.float().cpu()
 
     clocks = sampler.stop() if rank == 0 else None     # sampled across both device-timed regions (eager profile + graph)
     # ---------------- timed region 2: end to end through the public API with HOST buffers (pinned), H2D + D2H inside
@@ -405,17 +418,6 @@ def main():
         else:
             dom_name, d = "attn_tc_kernel", prof["attention"]
         ach = d["work_per_step"] / (d["ms_per_step"] / 1e3) / 1e12 if d["ms_per_step"] > 0 else 0.0
-        traffic, traffic_src = None, None
-        summ = os.path.join(ROOT, "profiles", "r02_launches_summary.json")
-        if not os.path.exists(summ):
-            summ = os.path.join(ROOT, "profiles", "r01_launches_summary.json")
-        if os.path.exists(summ):      # DRAM bytes per launch of the same kernel from the committed ncu capture of one step
-            with open(summ) as f:
-                ks = json.load(f)["kernels"]
-            sel = [v for k, v in ks.items() if k.startswith(dom_name.split(" ")[0])]
-            if sel:
-                traffic = sum((v["dram_read_MB"] + v["dram_write_MB"]) * 1e6 for v in sel) / sum(v["launches"] for v in sel)
-                traffic_src = f"profiles/{os.path.basename(summ)} (ncu dram__bytes_read.sum + dram__bytes_write.sum, cold L2)"
         kernels = {}
         for n, p_ in prof.items():
             if p_["ms_per_step"] <= 0:
@@ -430,14 +432,14 @@ def main():
         out = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": K, "warmup": W,
             "ms_per_step": ms / K, "higher_is_better": True, "scaling": "strong" if cfg_split else "weak", "vs_baseline": None, "dtype": "f16",
-            "data": "synthetic",
+            "data": "synthetic", "gpu": torch.cuda.get_device_name(dev),
             "config": {"workload": f"{Fr}-frame {8 * LH}x{8 * LW} (latent [1,4,{Fr},{LH},{LW}]), CFG 7.5 (UNet batch 2), ED-LoRA embeds "
                                    f"[2,16,77,768], adapter residuals active, DDIM step; " +
                                    (f"ONE video over {world} GPUs: CFG halves x {plan.frame_shards} frame shard(s); exchanges per step: 1 all-gather of eps"
                                     + (", 45 GroupNorm-statistics all-reduces, 40 frames<->pixels all-to-alls (NCCL, inside the CUDA graph)" if plan.frame_shards > 1 else "")
                                     if sharded else "one video per GPU"),
                        "parallelism": (f"cfg2 x frames{plan.frame_shards}" if sharded else f"replicas x{world}"),
-                       "timing": "CUDA events; working set (2.55 GB weights + activations) >> 126 MB L2, no flush needed; "
+                       "timing": "CUDA events; working set (2.55 GB weights + activations) >> 50 MB L2, no flush needed; "
                                  "`value`/`e2e` replay the step as a CUDA graph, the per-kernel profile comes from an eager pass "
                                  "of the same K steps with per-launch events",
                        "eager_ms_per_step": round(ms_eager / K, 3), "cuda_graph": gstep is not None,
@@ -448,7 +450,7 @@ def main():
             "gpu_launches": int(launches),
             "clocks": clocks,
             "roofline": {"kernel": dom_name, "bound": "tensor", "achieved": ach, "peak": pk["tflops"], "unit": "TFLOP/s",
-                         "frac": ach / pk["tflops"], "traffic": traffic, "traffic_source": traffic_src,
+                         "frac": ach / pk["tflops"],
                          "launches_per_step": d["launches_per_step"],
                          "flops_per_launch": d["work_per_step"] / max(d["launches_per_step"], 1),
                          "avg_launch_us": 1e3 * d["ms_per_step"] / max(d["launches_per_step"], 1), "peak_source": pk["source"]},
@@ -464,6 +466,10 @@ def main():
                                    "sample": f"oracle UNet fwd fp32 on [1,4,2,64,64] (1/16 CFG step), median of {len(times)} reps = {tmed:.2f} s"}
         else:
             out["cpu_baseline"] = None
+        if args.dump_outputs:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "latents.npy"), timed_out.numpy())
         print(json.dumps(out))
     if world > 1:
         dist.destroy_process_group()

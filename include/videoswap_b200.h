@@ -1,4 +1,4 @@
-/* videoswap_b200 -- C ABI of the B200-native denoising hot path of showlab/VideoSwap.
+/* videoswap_b200 -- C ABI of the H100-native denoising hot path of showlab/VideoSwap.
  *
  * The reference has no FFI boundary (it is pure Python on PyTorch/diffusers); its seam for this path is the Python
  * call  AnimateDiffUNet3DModel.forward  (videoswap/models/animatediff_models/unet.py:328-481)  plus the CFG combine and
@@ -200,41 +200,17 @@ int vs_profile_collect(int category, double* ms, double* work, long long* count)
 long long vs_launch_count(void);   /* kernels launched by this library since load */
 int vs_profile_dump(const char* path);   /* CSV: category, shape (m,n,k), work per launch, launches, total ms */
 /* Runtime A/B switches (defaults = the shipped configuration; unknown names are an error):
- *   "attn_tc"      1  tcgen05/TMEM attention kernel for head dims 40/80; 0 forces the mma.sync kernel
- *   "attn_handoff" 1  softmax warpgroups hand the MUFU pipe over after 7 of 8 key chunks; 0 = after the last one
- *   "gemm_pair"    1  CTA pairs (cta_group::2, 256-row tiles) for K >= 768; 0 = never; 2 = whenever >= 2 row tiles
+ *   "attn_tc"      1  wgmma/TMA attention kernel for head dims 40/80; 0 forces the mma.sync kernel
  *   "gemm_stages"  0  limit of the shared-memory ring depth of the GEMM (0 = as many as fit)
- *   "attn_persist" 1  persistent tcgen05 attention (one CTA per SM walks the work items, Q K^T and P V issued by two
- *                     warps); 0 = the round-1 kernel (one CTA per work item, one issuer warp)
- *   "attn_epiwg"   1  persistent d = 40 kernel: dedicated epilogue warpgroup, O accumulators double-buffered in TMEM
- *   "attn_pingpong" 1 persistent kernel: the two softmax warpgroups take turns on the MUFU pipe; 0 = free-running
- *   "attn_ptmem"   1  persistent kernel: the probabilities reach the P V MMA through tensor memory (tcgen05.st, A operand
- *                     from TMEM); 0 = through 128B-swizzled shared memory + generic->async proxy fence
- *   "attn_debug"   0  1 = the persistent d = 40 kernel records cycle counters (vs_debug_read)
- *   "attn_poly"    1  P chunks (of 8 per key tile) whose exp2 runs on the FMA pipe instead of MUFU.EX2 (0..3); 1 of 8 measured
- *                     neutral at full clocks and -10 % on a power-capped box (profiles/r02_attn_ab_*.json)
  *   "ln_fold"      1  LayerNorms folded into the consuming GEMM; 0 = stand-alone LayerNorm kernel
  *   "ln_fuse"      1  row statistics of folded LayerNorms written by the producing GEMM's epilogue; 0 = ln_stats pass
  *   "tattn_vst"    1  temporal attention writes its outputs with 16-byte stores from a shared-memory stage; 0 = 4-byte stores
  *   "gn_fused"     1  per-frame GroupNorms (Transformer3DModel.norm, motion-module norm) as ONE pass with the image resident
- *                     in the shared memory of a thread-block cluster where that measured faster (<= 4 CTAs x 160 KB: the
- *                     16x16 / 8x8 levels); 2 = up to 16 CTAs; 0 = statistics + apply kernels everywhere
+ *                     in the shared memory of a thread-block cluster (up to 16 CTAs x 160 KB); 0 = statistics + apply kernels
  *   "subpixel"     1  nearest-2x + conv3x3 as four sub-pixel convs; 0 = materialise the up-sampled tensor, then conv3x3
  *   "gn_stats_v2"  0  1 = GroupNorm statistics kernel with per-position accumulators instead of a per-element group select (no gain)
- *   "res_stage"    1  single-CTA linear layers with a residual and K <= 320 (proj_out / to_out at the 64x64 level): the epilogue
- *                     keeps the residual rows of a whole tile in shared memory, copied in with cp.async one tile ahead
- *                     (-8 % at M = 131072; deeper K loses more to the shorter operand ring than it gains); 0 = registers only
- *   "res_prefetch" 0  1 / 2 = residual rows of the next tile prefetched into L2 (prefetch.global.L2 / cp.async.bulk.prefetch.L2);
- *                     measured: no gain
- *   "epi_prefetch" 0  1 = GEMM / conv epilogue issues the TMEM load of sub-tile s+1 while sub-tile s is processed
- *                     (measured: GEMM time 21.6 -> 21.9 ms, no gain)
  *   "pdl"          1  programmatic dependent launch between the hot kernels; 0 = plain stream order */
 int vs_set_option(const char* name, int value);
-/* Cycle counters of the instrumented attention kernel (option "attn_debug" = 1): per CTA 16 values -- softmax warp 4:
- * total, wait for S (tiles > 0), wait for the MUFU turn, wait for the P buffer / rescale, exponential phase, epilogue, wait
- * for S (first tile of an item), key tiles; issuer warps: P V total, Q K^T wait Q, Q K^T wait K/V, P V wait P(tile 0), P V wait P(tile 1), wait V
- * ones column, wait O buffer, Q K^T wait for a free S buffer.  Synchronises the device.  Diagnostic only. */
-int vs_debug_read(unsigned long long* host_out, int n);
 
 #ifdef __cplusplus
 }

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.  Generates tests/golden/*.pt by running the REFERENCE's own model files
-(/root/reference, through oracle/diffusers_stub) on seeded inputs and seeded weights
-(videoswap_b200.weights.seeded_state_dict).  Run in the authoring container:  python -m oracle.make_golden
-The fixtures pin oracle/unet3d_oracle.py (tests/test_oracle_golden.py) wherever /root/reference is absent."""
+(a checkout of the reference, through oracle/diffusers_stub) on seeded inputs and seeded weights
+(videoswap_b200.weights.seeded_state_dict).  Run where the reference tree is checked out:  python -m oracle.make_golden
+The fixtures pin oracle/unet3d_oracle.py (tests/test_oracle_golden.py) wherever the reference is absent."""
 import os
 import sys
 
@@ -78,8 +78,7 @@ def run_adapter():
     emb = randn((6, 1280), 6)
     with torch.no_grad():
         maps = ad(tracks[None], (128, 128), emb[None], index_list=None)
-    torch.save({"tracks": tracks, "emb": emb, "size": (128, 128), "maps": [m.contiguous() for m in maps]},
-               os.path.join(OUT, "adapter.pt"))
+    torch.save({"tracks": tracks, "emb": emb, "size": (128, 128), "maps_sparse": sparsify(maps)}, os.path.join(OUT, "adapter.pt"))
     print("adapter", [tuple(m.shape) for m in maps], [float(m.abs().sum()) for m in maps])
 
 
@@ -95,6 +94,15 @@ def adapter_fp16_inputs():
     tracks[4, 4] = torch.tensor([700.77, 13.31])
     emb = randn((8, 1280), 16)
     return tracks, emb, (768, 448), [0, 1, 2, 3, 4, 6, 7]
+
+
+def sparsify(maps):
+    """The maps are zero except around the points: (frame, y, x) of the non-zero cells and their channel vectors."""
+    sparse = []
+    for m in maps:
+        idx = (m != 0).any(dim=1).nonzero()
+        sparse.append({"shape": tuple(m.shape), "idx": idx.to(torch.int32), "val": m[idx[:, 0], :, idx[:, 1], idx[:, 2]].contiguous()})
+    return sparse
 
 
 def densify(sparse):
@@ -119,12 +127,7 @@ def run_adapter_fp16():
     with torch.no_grad():
         maps = ad(tracks[None].half(), size, emb[None].half(), index_list=index_list)
     assert all(m.dtype == torch.float16 for m in maps)
-    # the maps are zero except around the points: store (frame, y, x) of the non-zero cells and their channel vectors
-    sparse = []
-    for m in maps:
-        idx = (m != 0).any(dim=1).nonzero()
-        sparse.append({"shape": tuple(m.shape), "idx": idx.to(torch.int32), "val": m[idx[:, 0], :, idx[:, 1], idx[:, 2]].contiguous()})
-    torch.save({"maps_sparse": sparse}, os.path.join(OUT, "adapter_fp16.pt"))
+    torch.save({"maps_sparse": sparsify(maps)}, os.path.join(OUT, "adapter_fp16.pt"))
     print("adapter_fp16", [tuple(m.shape) for m in maps], [float(m.float().abs().sum()) for m in maps])
 
 

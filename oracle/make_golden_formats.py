@@ -1,10 +1,10 @@
 """TEST INFRASTRUCTURE ONLY.  Golden vectors for videoswap_b200/formats.py (SURVEY.md 8f-4, data formats), produced by the
-REFERENCE's own functions read from /root/reference:
+REFERENCE's own functions read from the reference checkout:
 
   merge_lora_into_weight   utils/convert_edlora_to_diffusers.py:36-81   (module imports only `copy`: loaded as a file)
   select_frame_idx         data/frame_point_dataset.py:13-22            } their modules import PIL / torchvision / CLIP, so the
   bind_concept_prompt      utils/edlora_util.py:100-111                 } single function is compiled from the file's AST
-                                                                          (executed from /root/reference, nothing is copied)
+                                                                          (executed from the reference checkout, nothing is copied)
 
 The UNet state dict is the seeded tiny configuration of the CPU tests (re-created from its seed by the test, not stored); the
 fixture stores the LoRA, and for the merged result the touched tensors of a few named keys plus a digest over all of them.
@@ -20,7 +20,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 OUT = os.path.join(ROOT, "tests", "golden", "formats.pt")
-REF = os.environ.get("VIDEOSWAP_REFERENCE", "/root/reference")
+REF = os.environ.get("VIDEOSWAP_REFERENCE", "")      # a checkout of showlab/VideoSwap (required)
 
 TINY = dict(boc=(32, 64, 128, 128), ctx=64, groups=8)
 RANK, ALPHA = 4, 0.6
@@ -75,6 +75,8 @@ def digest(sd, keys):
 
 
 def main():
+    if not os.path.isfile(os.path.join(REF, "videoswap/utils/convert_edlora_to_diffusers.py")):
+        sys.exit("set VIDEOSWAP_REFERENCE to a checkout of showlab/VideoSwap")
     spec = importlib.util.spec_from_file_location("ref_convert_edlora", os.path.join(REF, "videoswap/utils/convert_edlora_to_diffusers.py"))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)

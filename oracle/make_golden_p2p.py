@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY.  Golden vectors for the attention controllers (SURVEY.md 8f-2), produced by the REFERENCE's own
 classes -- utils/p2p_utils/attention_store.AttentionStore, attention_util.make_controller -> AttentionRefine /
-AttentionReplace, spatial_blend.SpatialBlender -- imported unmodified from /root/reference (through oracle/diffusers_stub;
+AttentionReplace, spatial_blend.SpatialBlender -- imported unmodified from the reference checkout (through oracle/diffusers_stub;
 a whitespace tokenizer stands in for CLIP's, it only drives the reference's own word alignment).
 
 Scenario (everything seeded): an inversion pass stores the maps / latents of N steps (LOW_RESOURCE, batch = F frames), then an

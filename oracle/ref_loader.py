@@ -1,23 +1,24 @@
-"""TEST INFRASTRUCTURE ONLY.  Imports the reference's OWN model files, unmodified, from /root/reference
-through oracle/diffusers_stub (the reference's `diffusers==0.19.3` dependency is not installable offline).
-Only usable in the authoring container (/root/reference does not exist on the GPU box); used by
-oracle/make_golden.py to pin oracle/unet3d_oracle.py and by tests that skip when the reference is absent."""
+"""TEST INFRASTRUCTURE ONLY.  Imports the reference's OWN model files, unmodified, from a checkout of showlab/VideoSwap
+named by the environment variable VIDEOSWAP_REFERENCE, through oracle/diffusers_stub (the reference's `diffusers==0.19.3`
+dependency is not installable offline).  Used by the golden-fixture generators (oracle/make_golden*.py); the tests only
+read the fixtures they wrote."""
 import importlib
 import os
 import sys
 
-REFERENCE_ROOT = os.environ.get("VIDEOSWAP_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("VIDEOSWAP_REFERENCE", "")
 _STUB = os.path.join(os.path.dirname(os.path.abspath(__file__)), "diffusers_stub")
 
 
 def reference_available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "videoswap", "models", "animatediff_models"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "videoswap", "models", "animatediff_models"))
 
 
 def load_reference():
     """Returns a namespace with the reference classes (AnimateDiffUNet3DModel, SparsePointAdapter, ...)."""
     if not reference_available():
-        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT}")
+        raise RuntimeError("set VIDEOSWAP_REFERENCE to a checkout of showlab/VideoSwap"
+                           + (f" (no reference model files under {REFERENCE_ROOT})" if REFERENCE_ROOT else ""))
     try:
         import diffusers  # noqa: F401
         if "stub" not in getattr(diffusers, "__version__", ""):

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY (never imported by videoswap_b200/): CPU fp32 restatement of the reference's
 per-timestep denoising path, written functionally over a flat diffusers-style state_dict.
 
-Follows (reference file:line, relative to /root/reference):
+Follows (reference file:line, relative to the reference repository):
   * AnimateDiffUNet3DModel.forward            videoswap/models/animatediff_models/unet.py:328-481
   * block containers                          .../unet_blocks.py:258-265, 366-412, 480-508, 605-651, 715-740
   * ResnetBlock3D / Up/Downsample3D           .../resnet.py:163-193, 21-95   (5-D GroupNorm couples frames)
@@ -15,7 +15,7 @@ Follows (reference file:line, relative to /root/reference):
     -- restated from the published algorithm.
 
 Pinning: the reference ships no tests/golden vectors (SURVEY.md section 4), so this oracle is pinned against the
-reference's OWN model files executed in the authoring container through oracle/diffusers_stub (see
+reference's OWN model files executed from a checkout of the reference through oracle/diffusers_stub (see
 oracle/make_golden.py -> tests/golden/*.pt).  The diffusers pieces themselves remain "parity unpinned"
 (no diffusers install is available offline); DESIGN.md states this.
 """

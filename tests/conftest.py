@@ -10,9 +10,8 @@ if ROOT not in sys.path:
 
 def pytest_configure(config):
     import torch
-    torch.set_num_threads(min(os.cpu_count() or 1, 16))   # the CPU oracle is slowest with all 128 threads of the GPU box
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
-    config.addinivalue_line("markers", "reference: needs /root/reference (authoring container only)")
+    torch.set_num_threads(min(os.cpu_count() or 1, 16))   # the CPU oracle gets slower beyond ~16 threads
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -269,7 +269,7 @@ def check_self_attention(B=3, N=200, C=320, seed=120):
 
 
 def check_self_attention_mma(**kw):
-    """Same problem on the mma.sync kernel (the tcgen05 kernel is the default for d = 40 / 80)."""
+    """Same problem on the mma.sync kernel (the wgmma kernel is the default for d = 40 / 80)."""
     ops.set_option("attn_tc", 0)
     try:
         return check_self_attention(**kw)
@@ -324,67 +324,63 @@ CHECKS = {
     "gemm_bn256_res": lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, seed=8),
     "gemm_bn256_forced_tail": lambda: check_gemm(700, 768, 640, bn=256, seed=9),
     "conv_bn256": lambda: check_conv3x3(n=16, H=32, W=32, ci=320, co=1280, rowvec=True, residual=True),
-    # CTA pairs (cta_group::2) are the default for >= 2 row tiles: odd row-tile counts (dummy second tile), ragged M,
-    # and the single-CTA kernels behind the "gemm_pair" = 0 switch
+    # odd row-tile counts, ragged M, small and large K, GEGLU, conv and concat shapes
     "gemm_pair_odd_m": lambda: check_gemm(128 * 3, 640, 1280, residual=True, seed=12),
     "gemm_pair_ragged_m": lambda: check_gemm(128 * 5 + 9, 1280, 1024, seed=13),
-    "gemm_pair_small_k": with_option("gemm_pair", 2, lambda: check_gemm(128 * 7 + 3, 960, 320, seed=14), 1),
-    "geglu_pair_small_k": with_option("gemm_pair", 2, lambda: check_geglu(M=1000, C=320, seed=33), 1),
+    "gemm_pair_small_k": lambda: check_gemm(128 * 7 + 3, 960, 320, seed=14),
+    "geglu_pair_small_k": lambda: check_geglu(M=1000, C=320, seed=33),
     "conv_pair_odd": lambda: _conv_odd(3, 7, 12, 320, 320, 56),
-    "single_gemm": with_option("gemm_pair", 0, lambda: check_gemm(1024, 1280, 1280, residual=True, seed=7), 1),
-    "single_gemm_bn256": with_option("gemm_pair", 0, lambda: check_gemm(8192, 3840, 640, seed=7), 1),
-    "single_geglu": with_option("gemm_pair", 0, lambda: check_geglu(M=1000, C=640, seed=32), 1),
-    "single_conv": with_option("gemm_pair", 0, lambda: check_conv3x3(rowvec=True, residual=True), 1),
-    "single_concat": with_option("gemm_pair", 0, check_gemm_concat, 1),
-    # tile counts that leave one epilogue warpgroup (accumulator stage) without work on some CTAs
+    "single_gemm": lambda: check_gemm(1024, 1280, 1280, residual=True, seed=7),
+    "single_gemm_bn256": with_option("gemm_stages", 3, lambda: check_gemm(8192, 3840, 640, seed=7), 0),
+    "single_geglu": lambda: check_geglu(M=1000, C=640, seed=32),
+    "single_conv": with_option("gemm_stages", 3, lambda: check_conv3x3(rowvec=True, residual=True), 0),
+    "single_concat": with_option("gemm_stages", 3, lambda: check_gemm_concat(), 0),
+    # tile counts that leave some CTAs of the persistent grid without work, or with one tile more than others
     "gemm_one_tile": lambda: check_gemm(100, 128, 64, seed=10),
     "gemm_149_tiles": lambda: check_gemm(128 * 149, 128, 128, residual=True, seed=11),
-    # tcgen05 attention variants kept for A/B measurements: late hand-over of the MUFU pipe
-    "self_attn_d40_late_handoff": with_option("attn_handoff", 0, lambda: check_self_attention(B=2, N=600, C=320, seed=121), 1),
-    # round-1 kernel (one CTA per work item) kept behind "attn_persist" = 0; FMA-pipe exponentials ("attn_poly") on the
-    # persistent kernel; more work items than SMs so that every CTA walks several items (148 SMs: 2*8*24 = 384 items)
-    "self_attn_d40_nonpersistent": with_option("attn_persist", 0, lambda: check_self_attention(B=2, N=600, C=320, seed=121), 1),
-    "self_attn_d80_nonpersistent": with_option("attn_persist", 0, lambda: check_self_attention(B=2, N=300, C=640, seed=123), 1),
-    "self_attn_d40_persistent_n4096": with_option("attn_persist", 2, lambda: check_self_attention(B=2, N=4096, C=320, seed=124), 1),
-    "self_attn_d40_poly2": with_option("attn_persist", 2, with_option("attn_poly", 2, lambda: check_self_attention(B=2, N=4096, C=320, seed=124), 1), 1),
-    "self_attn_d40_poly3": with_option("attn_persist", 2, with_option("attn_poly", 3, lambda: check_self_attention(B=3, N=700, C=320, seed=127), 1), 1),
-    "self_attn_d80_poly2": with_option("attn_poly", 2, lambda: check_self_attention(B=2, N=1024, C=640, seed=126), 1),
-    # P handed to the P V MMA through tensor memory (tcgen05.st, A operand from TMEM) instead of shared memory
-    # (default since r02k; the shared-memory P path stays behind "attn_ptmem" = 0)
-    "self_attn_d40_psmem": with_option("attn_ptmem", 0, lambda: check_self_attention(B=2, N=4096, C=320, seed=124), 1),
-    "self_attn_d40_psmem_ragged": with_option("attn_ptmem", 0, lambda: check_self_attention(B=3, N=700, C=320, seed=127), 1),
-    "self_attn_d80_psmem": with_option("attn_ptmem", 0, lambda: check_self_attention(B=2, N=1100, C=640, seed=129), 1),
-    "cross_attn_d40_psmem": with_option("attn_ptmem", 0, lambda: check_cross_attention(B=2, Fr=4, N=1024, C=320, seed=134), 1),
-    "cross_attn_d80_psmem": with_option("attn_ptmem", 0, lambda: check_cross_attention(B=2, Fr=8, N=1024, C=640, seed=133), 1),
-    "self_attn_d40_mufu_only": with_option("attn_poly", 0, lambda: check_self_attention(B=2, N=1024, C=320, seed=122), 1),
-    "self_attn_d40_free_running": with_option("attn_pingpong", 0, lambda: check_self_attention(B=2, N=1024, C=320, seed=122), 1),
-    "self_attn_d40_softmax_epilogue": with_option("attn_persist", 2, with_option("attn_epiwg", 0, lambda: check_self_attention(B=2, N=4096, C=320, seed=124), 1), 1),
-    "cross_attn_d40_softmax_epilogue": with_option("attn_epiwg", 0, lambda: check_cross_attention(B=2, Fr=4, N=1024, C=320, seed=134), 1),
-    "self_attn_d40_many_items": with_option("attn_persist", 2, lambda: check_self_attention(B=2, N=6144, C=320, seed=128), 1),
+    # tensor-core attention: ragged query / key counts, many query blocks and key tiles, both head dims, cross-attention.
+    # These ids (and the *_prefetch / *_respf* / *_resst* / *_pair* / single_* GEMM ids) come from the A/B switches of the
+    # previous kernel generation and are kept as ids; each now runs its own configuration: the mma.sync attention path
+    # ("attn_tc" = 0), a shallower GEMM operand ring ("gemm_stages" = 3 / 4), or another seed / ragged shape.
+    "self_attn_d40_late_handoff": lambda: check_self_attention(B=2, N=601, C=320, seed=125),
+    "self_attn_d40_nonpersistent": with_option("attn_tc", 0, lambda: check_self_attention(B=2, N=600, C=320, seed=121), 1),
+    "self_attn_d80_nonpersistent": with_option("attn_tc", 0, lambda: check_self_attention(B=2, N=300, C=640, seed=123), 1),
+    "self_attn_d40_persistent_n4096": lambda: check_self_attention(B=3, N=4096, C=320, seed=132),
+    "self_attn_d40_poly2": with_option("attn_tc", 0, lambda: check_self_attention(B=2, N=4096, C=320, seed=124), 1),
+    "self_attn_d40_poly3": lambda: check_self_attention(B=3, N=700, C=320, seed=127),
+    "self_attn_d80_poly2": with_option("attn_tc", 0, lambda: check_self_attention(B=2, N=1024, C=640, seed=126), 1),
+    "self_attn_d40_psmem": lambda: check_self_attention(B=1, N=4096, C=320, seed=130),
+    "self_attn_d40_psmem_ragged": with_option("attn_tc", 0, lambda: check_self_attention(B=3, N=700, C=320, seed=127), 1),
+    "self_attn_d80_psmem": lambda: check_self_attention(B=2, N=1100, C=640, seed=129),
+    "cross_attn_d40_psmem": lambda: check_cross_attention(B=2, Fr=4, N=1024, C=320, seed=134),
+    "cross_attn_d80_psmem": with_option("attn_tc", 0, lambda: check_cross_attention(B=2, Fr=8, N=1024, C=640, seed=133), 1),
+    "self_attn_d40_mufu_only": lambda: check_self_attention(B=2, N=1024, C=320, seed=122),
+    "self_attn_d40_free_running": with_option("attn_tc", 0, lambda: check_self_attention(B=2, N=1024, C=320, seed=122), 1),
+    "self_attn_d40_softmax_epilogue": lambda: check_self_attention(B=2, N=4095, C=320, seed=131),
+    "cross_attn_d40_softmax_epilogue": with_option("attn_tc", 0, lambda: check_cross_attention(B=2, Fr=4, N=1024, C=320, seed=134), 1),
+    "self_attn_d40_many_items": lambda: check_self_attention(B=2, N=6144, C=320, seed=128),
     "self_attn_d80_many_items_odd_tiles": lambda: check_self_attention(B=6, N=1100, C=640, seed=129),     # nkt = 18, 5 q blocks
     "cross_attn_d80_many_items": lambda: check_cross_attention(B=2, Fr=8, N=1024, C=640, seed=133),
-    # epilogue with the TMEM load of the next sub-tile in flight ("epi_prefetch" = 1)
-    "gemm_bn160_prefetch": with_option("epi_prefetch", 1, lambda: check_gemm(512, 320, 320), 0),
-    "gemm_residual_prefetch": with_option("epi_prefetch", 1, lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, seed=8), 0),
-    "gemm_pair_prefetch": with_option("epi_prefetch", 1, lambda: check_gemm(128 * 5 + 9, 1280, 1024, seed=13), 0),
-    "conv3x3_epi_prefetch": with_option("epi_prefetch", 1, lambda: check_conv3x3(rowvec=True, residual=True), 0),
-    "ln_fuse_res_prefetch": with_option("epi_prefetch", 1, lambda: check_linear_ln_linear(rows=128 * 150 + 37, residual=True, N=320, seed=161, mean=2.0), 0),
-    "gemm_bn128_tail_prefetch": with_option("epi_prefetch", 1, lambda: check_gemm(300, 768, 320, bn=128), 0),
-    # residual rows of the next tile prefetched into L2 ("res_prefetch": 1 = prefetch.global.L2, 2 = cp.async.bulk.prefetch.L2);
-    # ragged M (rows outside the problem must not be touched), partial last column tile, conv geometry, CTA pairs
-    "gemm_residual_respf1": with_option("res_prefetch", 1, lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, seed=8), 0),
-    "gemm_residual_respf2": with_option("res_prefetch", 2, lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, seed=8), 0),
-    "gemm_residual_k320_respf1": with_option("res_prefetch", 1, lambda: check_gemm(128 * 301 + 77, 320, 320, residual=True, seed=21), 0),
-    "gemm_residual_k320_respf2": with_option("res_prefetch", 2, lambda: check_gemm(128 * 301 + 77, 320, 320, residual=True, seed=21), 0),
-    "gemm_residual_n96_respf2": with_option("res_prefetch", 2, lambda: check_gemm(128 * 3 + 5, 96, 320, residual=True, seed=22), 0),
-    "gemm_pair_residual_respf1": with_option("res_prefetch", 1, lambda: check_gemm(128 * 5 + 9, 1280, 1024, residual=True, seed=13), 0),
-    "gemm_pair_residual_respf2": with_option("res_prefetch", 2, lambda: check_gemm(128 * 5 + 9, 1280, 1024, residual=True, seed=13), 0),
-    "conv3x3_respf1": with_option("res_prefetch", 1, lambda: check_conv3x3(rowvec=True, residual=True), 0),
-    "conv3x3_respf2": with_option("res_prefetch", 2, lambda: check_conv3x3(rowvec=True, residual=True), 0),
-    "ln_fuse_res_respf2": with_option("res_prefetch", 2, lambda: check_linear_ln_linear(rows=128 * 150 + 37, residual=True, N=320, seed=161, mean=2.0), 0),
-    # whole-tile residual stage in shared memory ("res_stage" = 1, default; single-CTA linear layers with K <= 320): many tiles
-    # per CTA (refill of consumed chunks with the next tile's rows), ragged M, a partial last column tile (different sub-tile
-    # counts of consecutive tiles), every BN that takes the path, the K boundary, and the register path kept for A/B
+    # epilogue sub-tile counts, residual adds and partial column tiles at several BN
+    "gemm_bn160_prefetch": with_option("gemm_stages", 3, lambda: check_gemm(512, 320, 320), 0),
+    "gemm_residual_prefetch": with_option("gemm_stages", 4, lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, seed=8), 0),
+    "gemm_pair_prefetch": with_option("gemm_stages", 3, lambda: check_gemm(128 * 5 + 9, 1280, 1024, seed=13), 0),
+    "conv3x3_epi_prefetch": with_option("gemm_stages", 4, lambda: check_conv3x3(rowvec=True, residual=True), 0),
+    "ln_fuse_res_prefetch": with_option("gemm_stages", 3, lambda: check_linear_ln_linear(rows=128 * 150 + 37, residual=True, N=320, seed=161, mean=2.0), 0),
+    "gemm_bn128_tail_prefetch": with_option("gemm_stages", 4, lambda: check_gemm(300, 768, 320, bn=128), 0),
+    # residual epilogue: ragged M (rows outside the problem must not be touched), partial last column tile, conv geometry
+    "gemm_residual_respf1": with_option("gemm_stages", 3, lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, seed=8), 0),
+    "gemm_residual_respf2": lambda: check_gemm(128 * 150 + 9, 1280, 320, residual=True, bn=128, seed=18),
+    "gemm_residual_k320_respf1": with_option("gemm_stages", 3, lambda: check_gemm(128 * 301 + 77, 320, 320, residual=True, seed=21), 0),
+    "gemm_residual_k320_respf2": with_option("gemm_stages", 4, lambda: check_gemm(128 * 301 + 77, 320, 320, residual=True, seed=21), 0),
+    "gemm_residual_n96_respf2": lambda: check_gemm(128 * 3 + 5, 96, 320, residual=True, seed=22),
+    "gemm_pair_residual_respf1": with_option("gemm_stages", 3, lambda: check_gemm(128 * 5 + 9, 1280, 1024, residual=True, seed=13), 0),
+    "gemm_pair_residual_respf2": with_option("gemm_stages", 4, lambda: check_gemm(128 * 5 + 9, 1280, 1024, residual=True, seed=13), 0),
+    "conv3x3_respf1": lambda: check_conv3x3(n=4, H=24, W=40, rowvec=True, residual=True, seed=41),
+    "conv3x3_respf2": lambda: check_conv3x3(n=2, H=32, W=32, ci=640, co=640, rowvec=True, residual=True, seed=42),
+    "ln_fuse_res_respf2": with_option("gemm_stages", 4, lambda: check_linear_ln_linear(rows=128 * 150 + 37, residual=True, N=320, seed=161, mean=2.0), 0),
+    # residual epilogue with many tiles per CTA, ragged M, a partial last column tile (different sub-tile counts of
+    # consecutive tiles), every BN, and short to long K
     "gemm_resst_l0_full": lambda: check_gemm(131072, 320, 320, residual=True, seed=31),
     "gemm_resst_ragged_many_tiles": lambda: check_gemm(128 * 901 + 77, 320, 320, residual=True, seed=32),
     "gemm_resst_n96_partial_tile": lambda: check_gemm(128 * 40 + 5, 96, 320, residual=True, seed=33),
@@ -395,9 +391,9 @@ CHECKS = {
     "gemm_res_k384_register_path": lambda: check_gemm(4096, 320, 384, residual=True, seed=38),
     "gemm_res_k1280_register_path": lambda: check_gemm(32768, 320, 1280, residual=True, seed=40),
     "gemm_res_pair_k1024_register_path": lambda: check_gemm(128 * 64 + 9, 1280, 1024, residual=True, seed=39),
-    "gemm_resst_off_register_path": with_option("res_stage", 0, lambda: check_gemm(128 * 301 + 77, 320, 320, residual=True, seed=21), 1),
+    "gemm_resst_off_register_path": lambda: check_gemm(128 * 302 + 1, 320, 320, residual=True, seed=23),
     "ln_fuse_res_resst_many_tiles": lambda: check_linear_ln_linear(rows=128 * 700 + 37, residual=True, N=320, seed=162, mean=2.0),
-    "ln_fuse_res_resst_off": with_option("res_stage", 0, lambda: check_linear_ln_linear(rows=128 * 150 + 37, residual=True, N=320, seed=161, mean=2.0), 1),
+    "ln_fuse_res_resst_off": lambda: check_linear_ln_linear(rows=128 * 151 + 5, residual=True, N=320, seed=165, mean=-2.0),
     "gemm_bn160": lambda: check_gemm(512, 320, 320),
     "gemm_bn128_tail": lambda: check_gemm(300, 768, 320, bn=128),
     "gemm_bn64": lambda: check_gemm(130, 64, 128, bn=64),
@@ -437,8 +433,8 @@ CHECKS = {
     "gn5d_c2_l0_mean3_stats_v2": with_option("gn_stats_v2", 1, lambda: check_groupnorm(B=2, Fr=16, H=64, W=64, c1=320, mean=3.0, seed=101), 0),
     # per-frame GroupNorm, single pass in a thread-block cluster: 16 / 8 / 4 / 1 CTAs per image, SiLU variant, and the
     # two-kernel path behind "gn_fused" = 0 (also taken when an image does not fit: 96x96 at 320 channels = 5.9 MB)
-    "gn_frame_fused_l1": with_option("gn_fused", 2, lambda: check_groupnorm(B=2, Fr=3, H=32, W=32, c1=640, per_frame=True, silu=False, eps=1e-6, mean=-1.0, seed=104), 1),
-    "gn_frame_fused_l0_cluster16": with_option("gn_fused", 2, lambda: check_groupnorm(B=2, Fr=4, H=64, W=64, c1=320, per_frame=True, silu=False, eps=1e-6, mean=2.0, seed=103), 1),
+    "gn_frame_fused_l1": with_option("gn_fused", 1, lambda: check_groupnorm(B=2, Fr=3, H=32, W=32, c1=640, per_frame=True, silu=False, eps=1e-6, mean=-1.0, seed=104), 1),
+    "gn_frame_fused_l0_cluster16": with_option("gn_fused", 1, lambda: check_groupnorm(B=2, Fr=4, H=64, W=64, c1=320, per_frame=True, silu=False, eps=1e-6, mean=2.0, seed=103), 1),
     "gn_frame_fused_l2": lambda: check_groupnorm(B=2, Fr=3, H=16, W=16, c1=1280, per_frame=True, silu=False, eps=1e-6, mean=0.5, seed=105),
     "gn_frame_fused_l3_silu": lambda: check_groupnorm(B=2, Fr=3, H=8, W=8, c1=1280, per_frame=True, silu=True, eps=1e-6, seed=106),
     "gn_frame_fused_odd": lambda: check_groupnorm(B=1, Fr=3, H=7, W=12, c1=320, per_frame=True, silu=False, eps=1e-6, seed=107),

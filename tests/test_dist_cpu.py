@@ -1,7 +1,8 @@
 """CPU tests of the multi-rank path (gloo, world_size 2 and 4): the rank plan, and -- with the oracle standing in for the
 CUDA kernels -- that the exchanges the frame-sharded / CFG-split step performs (GroupNorm-statistics all-reduce, frames <->
 pixels re-sharding around the motion modules, all-gather of the two noise predictions) reproduce the single-process
-step.  The CUDA implementation of the same exchanges is checked on GPUs by tools/gpu_shard_check.py."""
+step.  The CUDA implementation of the same exchanges is checked on GPUs by tests/test_multi_gpu.py
+(tools/gpu_shard_check.py under torchrun)."""
 import os
 
 import torch

@@ -203,21 +203,23 @@ def adapter_fp16_vs_golden():
 
 
 def adapter_vs_golden():
+    from oracle.make_golden import densify
     g = torch.load(os.path.join(GOLD, "adapter.pt"))
+    ref = densify(g["maps_sparse"])
     ad = SparsePointAdapter(init="empty")
     ad.load_state_dict(seeded_state_dict(adapter_param_shapes(), seed=5))
     ad = ad.cuda()
     maps = ad(g["tracks"].cuda(), g["size"], g["emb"].cuda(), coord_fp16=False, as_nchw=True)
     torch.cuda.synchronize()
-    errs = [(m.float().cpu() - r).abs().max().item() for m, r in zip(maps, g["maps"])]
-    refs = [r.abs().max().item() for r in g["maps"]]
+    errs = [(m.float().cpu() - r).abs().max().item() for m, r in zip(maps, ref)]
+    refs = [r.abs().max().item() for r in ref]
     return {"errs": errs, "refs": refs}
 
 
 def edlora_merge_vs_oracle(Fr=2, hw=8, alpha=0.6, rank=4):
     """formats.merge_edlora_into_unet on the NATIVE model (parameters on the GPU, re-packed lazily) vs the oracle run on
     independently merged weights; then restore_unet brings the parameters back bit for bit (the OUTPUT is compared in dB: the
-    GroupNorm statistics use float atomics, so two forwards of the same weights agree to ~70 dB, not bit for bit: profiles/r02_edlora_merge.json)."""
+    GroupNorm statistics use float atomics, so two forwards of the same weights agree to ~70 dB, not bit for bit)."""
     from videoswap_b200 import formats
     m, sd = get_model()
     g = torch.Generator().manual_seed(77)

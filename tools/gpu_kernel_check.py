@@ -1,5 +1,5 @@
-"""Diagnostics for the GPU box: runs every kernel check in its own subprocess (a trapping kernel poisons the CUDA
-context, so isolation keeps the other results) and writes gpurun_out/kernel_check.json."""
+"""GPU diagnostics: runs every kernel check in its own subprocess (a trapping kernel poisons the CUDA
+context, so isolation keeps the other results); REPORT_JSON = path of a JSON report."""
 import json
 import os
 import subprocess
@@ -32,9 +32,9 @@ def main():
         except subprocess.TimeoutExpired:
             out[n] = {"ok": False, "timeout": True}
         print(n, out[n], flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "kernel_check.json"), "w") as f:
-        json.dump(out, f, indent=1)
+    if os.environ.get("REPORT_JSON"):            # optional: full JSON report to this path
+        with open(os.environ["REPORT_JSON"], "w") as f:
+            json.dump(out, f, indent=1)
     bad = [n for n, r in out.items() if not r.get("ok")]
     print(f"{len(out) - len(bad)}/{len(out)} ok; failing: {bad}")
 

@@ -1,4 +1,4 @@
-"""Evidence run for the attention controllers (SURVEY.md 8f-2) on the GPU box -> gpurun_out/r02_p2p_flow.json:
+"""Evidence run for the attention controllers (SURVEY.md 8f-2) (REPORT_JSON = path of a JSON report):
 explicit-probability attention vs torch, the hook vs the oracle's hook, the device-native controllers replayed against the
 fixtures the reference's own classes produced, the whole `use_blend: true` flow vs the oracle, and what controller mode costs
 per step at the benchmark size (eager, host callback per controlled layer) next to the CUDA-graph step."""
@@ -50,9 +50,9 @@ def main():
         out["stored_bytes_per_step"] = sum(t.numel() * t.element_size() for v in store.attention_store.values() for t in v) // 2
     finally:
         p2p.register_attention_control(pipe, None)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "r02_p2p_flow.json"), "w") as f:
-        json.dump(out, f, indent=1)
+    if os.environ.get("REPORT_JSON"):            # optional: full JSON report to this path
+        with open(os.environ["REPORT_JSON"], "w") as f:
+            json.dump(out, f, indent=1)
     print(json.dumps(out)[:3000])
 
 

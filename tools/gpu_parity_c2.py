@@ -1,7 +1,7 @@
 """Parity at the BENCHMARKED configuration (VERDICT r1, item 1): one full CFG denoise step on latents [1,4,16,64,64]
 (UNet batch 2, ED-LoRA embeddings [2,16,77,768], adapter residuals) through the native path -- eager AND the CUDA-graph
-replay bench.py times -- against the CPU fp32 oracle, with per-block taps.  ~3 min of CPU time on the GPU box.
-Writes gpurun_out/r02_unet_parity_c2.json (copied to profiles/ once reviewed)."""
+replay bench.py times -- against the CPU fp32 oracle, with per-block taps.  ~3 min of CPU time.
+With REPORT_JSON set, writes the full report (per-block taps) there."""
 import json
 import os
 import sys
@@ -74,9 +74,9 @@ def main():
     out["min_tap_psnr"] = min(v["psnr"] for v in taps.values()) if taps else None
     out["ok"] = bool(out["eps"]["finite"] and out["eps"]["psnr"] >= 40 and out["step_graph"]["psnr"] >= 40 and
                      (out["min_tap_psnr"] is None or out["min_tap_psnr"] >= 40))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "r02_unet_parity_c2.json"), "w") as f:
-        json.dump(out, f, indent=1)
+    if os.environ.get("REPORT_JSON"):            # optional: full JSON report to this path
+        with open(os.environ["REPORT_JSON"], "w") as f:
+            json.dump(out, f, indent=1)
     print(json.dumps({k: v for k, v in out.items() if k != "taps"}))
     sys.exit(0 if out["ok"] else 1)
 

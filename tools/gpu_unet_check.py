@@ -1,4 +1,4 @@
-"""Diagnostics for the GPU box: whole-UNet parity with per-stage taps -> gpurun_out/unet_check.json."""
+"""GPU diagnostics: whole-UNet parity with per-stage taps (REPORT_JSON = path of a JSON report)."""
 import json
 import os
 import sys
@@ -24,9 +24,9 @@ def main():
             import traceback
             out[name] = {"error": repr(e), "tb": traceback.format_exc()[-2000:]}
         print(name, json.dumps(out[name])[:3000], time.time() - t0, flush=True)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "unet_check.json"), "w") as f:
-        json.dump(out, f, indent=1)
+    if os.environ.get("REPORT_JSON"):            # optional: full JSON report to this path
+        with open(os.environ["REPORT_JSON"], "w") as f:
+            json.dump(out, f, indent=1)
 
 
 if __name__ == "__main__":

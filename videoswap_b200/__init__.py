@@ -1,4 +1,4 @@
-"""videoswap_b200: B200-native (sm_100a) implementation of the denoising hot path of showlab/VideoSwap -- the
+"""videoswap_b200: H100-native (sm_90a) implementation of the denoising hot path of showlab/VideoSwap -- the
 `AnimateDiffUNet3DModel` forward + classifier-free guidance + DDIM step -- behind the reference's own Python surface.
 See DESIGN.md / INTEGRATION.md.  Importing this package never touches `oracle/` and there is no CPU fallback."""
 from . import formats  # noqa: F401

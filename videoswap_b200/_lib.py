@@ -78,7 +78,6 @@ _SIGNATURES = {
     "vs_attention_apply_probs": (_I, [_P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _LL, _LL, _I]),
     "vs_blend_mask": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _I, _I, _F, _I, _P]),
     "vs_latent_blend": (_I, [_P, _P, _P, _P, _I, _I, _I, _I]),
-    "vs_debug_read": (_I, [C.POINTER(C.c_ulonglong), _I]),
     "vs_linear_ln_linear": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _I, _P]),
     "vs_attention": (_I, [_P, _P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _LL, _LL, _LL, _I]),
     "vs_temporal_attention": (_I, [_P, _P, _P, _I, _I, _I, _I, _I]),

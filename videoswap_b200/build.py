@@ -1,4 +1,4 @@
-"""In-tree build of libvideoswap_b200.so with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""In-tree build of libvideoswap_b200.so with nvcc for sm_90a (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvideoswap_b200.so")
 SOURCES = ["runtime.cu", "gemm.cu", "norm.cu", "attention.cu", "attention_tc.cu", "pointwise.cu", "unet.cu", "api.cu", "comm.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--use_fast_math" if False else "-DVS_NO_FAST_MATH"]
 
 
@@ -50,7 +51,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     if force or _stale(LIB, objs):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-ldl"]
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-Xcompiler", "-fPIC", "-ldl"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -131,11 +131,6 @@ extern "C" int vs_latent_blend(void* stream, const void* d_x_src, void* d_x_tgt,
                                int frames, int hw) {
   return latent_blend((cudaStream_t)stream, d_x_src, d_x_tgt, d_mask, io_f32, channels, frames, hw);
 }
-extern "C" int vs_debug_read(unsigned long long* host_out, int n) {
-  VS_REQUIRE(host_out && n > 0 && n <= 256 * 16, "vs_debug_read: bad arguments");
-  VS_REQUIRE(attention_debug_read(host_out, n) == 0, "vs_debug_read: no debug counters recorded (set option attn_debug)");
-  return 0;
-}
 extern "C" int vs_linear_ln_linear(void* stream, const void* d_x0, int M, int K0, const void* d_w0, const float* d_b0,
                                    const void* d_residual, int C, void* d_x, const void* d_w, const float* d_bias, int N,
                                    const float* d_gamma, const float* d_beta, int mode, void* d_wf, float* d_u, float* d_c,

@@ -5,7 +5,7 @@
 //  * temporal_attention():  attention across the F frames of every pixel (motion_module.py:305-335), one warp per
 //                           (batch, pixel, head); probabilities never touch HBM and no '(b f) d c <-> (b d) f c'
 //                           transposes are materialised.
-// These are the legacy-tensor-path (HMMA) baseline kernels; the tcgen05/TMEM version replaces the spatial one.
+// These are the legacy-tensor-path (HMMA) baseline kernels; the wgmma version (attention_tc.cu) replaces the spatial one for d = 40 / 80.
 #include "common.cuh"
 #include "kernels.h"
 

@@ -1,20 +1,13 @@
-// tcgen05 / TMEM flash attention for sm_100a (spatial self-attention N x N and cross-attention N x 77; d = 40 / 80).
+// wgmma / TMA flash attention for sm_90a (spatial self-attention N x N and cross-attention N x 77; d = 40 / 80).
 //
-// One CTA = (batch, head, 256 queries) = two 128-query tiles, each owned by one softmax warpgroup:
-//   warp 0      TMA producer: Q once (4-D descriptor [d, head, token, batch]; head dim 40 is zero-padded to 64 by TMA
-//               out-of-bounds fill), then a ring of 64-key K / V tiles
-//   warp 1      single-thread tcgen05.mma issuer:  S_i = Q_i K^T  (K-major x K-major, fp32 in TMEM)
-//                                                  O_i += P_i V   (P from shared memory, V as MN-major B operand)
-//   warp 2      TMEM allocator
-//   warps 4-7   softmax warpgroup of query tile 0 (thread = one query row, reads S with tcgen05.ld)
-//   warps 8-11  softmax warpgroup of query tile 1
-// S is DOUBLE-BUFFERED per query tile in TMEM and the issuer runs Q K^T two key tiles ahead; P is double-buffered in
-// shared memory, so a softmax warpgroup never waits for a tensor-core round trip.  The two softmax warpgroups PING-PONG
-// on the MUFU pipe through two 256-thread named barriers (one computes exponentials while the other loads / reduces /
-// packs / stores) -- at d = 40 the kernel is bound by the 16 ex2/clk/SM MUFU rate and the latency of each warp's serial
-// tile, not by the MMAs (see DESIGN.md).  The softmax keeps a *stale* running maximum and only rescales O (tcgen05.ld/st
-// round trip) when the true maximum grew by more than 2^8.  P is written to shared memory in the 128-byte-swizzled
-// K-major layout the MMA consumes; the row sum comes out of the P V MMA through a column of ones written into V.
+// One CTA = one warpgroup = (batch, head, 64 queries).  Thread 0 streams 64-key K / V tiles into a two-stage ring with
+// TMA (4-D descriptors [d, head, token, batch]; head dims are zero-padded to whole 64-column blocks by the TMA
+// out-of-bounds fill, which also zero-fills keys beyond nk and queries beyond nq):
+//   S = Q K^T   wgmma.m64n64k16, Q and K from 128-byte-swizzled shared memory (both K-major), fp32 in registers
+//   softmax     online, per row: max over the warp quad, exp2 of the scaled scores, lazy-free exact rescale of O and l
+//   O += P V    wgmma with the fp16 probabilities as the REGISTER A operand (the S accumulator layout of each warp is
+//               the A-fragment layout), V from shared memory as an MN-major B operand
+// Several CTAs share an SM (40-80 KB of shared memory each), so one CTA's softmax overlaps another one's MMAs and loads.
 //
 // Replaces diffusers AttnProcessor2_0 / EDLoRA_AttnProcessor.__call__ (reference utils/edlora_util.py:47-65,
 // models/animatediff_models/attention.py:229-241).
@@ -24,29 +17,20 @@
 namespace vs {
 namespace {
 
-constexpr int TQ = 128;              // queries per tile (= UMMA M)
-constexpr int BKV = 64;              // keys per tile (one 128-byte swizzle row of P)
-constexpr int ATT_THREADS = 384;
+constexpr int TQ = 64;               // queries per CTA (= wgmma M)
+constexpr int BKV = 64;              // keys per tile
+constexpr int ATT_THREADS = 128;
 
 template <int D>
 struct TCfg {
   static constexpr int NCB = (D + 63) / 64;            // 64-wide (128-byte) column blocks of Q/K/V tiles
   static constexpr int DPK = (D + 15) / 16 * 16;       // padded contraction length of Q K^T
-  // N of the P V MMA / O accumulator columns: d value columns + ONE extra column of ones written into the V tile, so
-  // that O[:, D] accumulates the softmax row sum on the tensor core (it is rescaled with O for free); the softmax
-  // warps then spend no instructions on it.  For d = 40 the column lives in the padding that exists anyway (48).
-  static constexpr int DPO = (D + 1 + 15) / 16 * 16;
-  static constexpr int ST = (D <= 64) ? 4 : 3;         // K/V ring stages (>= 3: K runs two tiles ahead of V)
-  static constexpr int Q_BYTES = 2 * NCB * TQ * 128;
-  static constexpr int KV_BLOCK_BYTES = BKV * 128;
-  static constexpr int KV_STAGE_BYTES = 2 * NCB * KV_BLOCK_BYTES;     // K then V
-  static constexpr int P_TILE_BYTES = TQ * 128;
-  static constexpr int SMEM = Q_BYTES + ST * KV_STAGE_BYTES + 4 * P_TILE_BYTES + 1024 + 256;   // P double-buffered
-  static constexpr int O_STRIDE = (DPO <= 64) ? 64 : 128;             // TMEM column stride between O_0 and O_1
-  static constexpr int S_COL = 0, O_COL = 4 * BKV;                    // S_{i,b} at (2 i + b) * BKV
-  static constexpr int TMEM_COLS = 512;
-  static_assert(4 * BKV + 2 * O_STRIDE <= 512, "TMEM budget");
-  static_assert(SMEM <= 227 * 1024, "shared memory budget");
+  static constexpr int BLOCK_BYTES = 64 * 128;         // one 64-row x 128-byte swizzled block
+  static constexpr int Q_BYTES = NCB * BLOCK_BYTES;
+  static constexpr int KV_STAGE_BYTES = 2 * NCB * BLOCK_BYTES;     // K then V
+  static constexpr int OREG = (D > 64) ? 32 + 8 : 32;               // O accumulator: one n64 block (+ one n16 block)
+  static constexpr int SMEM = Q_BYTES + 2 * KV_STAGE_BYTES + 1024 + 64;
+  static_assert(D == 40 || D == 80, "head dims of the tensor-core path");
 };
 
 struct TAttnArgs {
@@ -56,763 +40,150 @@ struct TAttnArgs {
   long long o_bs;
   int nq, nk, kv_div;
   float scale_log2;
-  int heads, n_qblk, n_items;   // persistent kernel: work item = (batch, head, 256-query block), q block fastest
-  unsigned long long* dbg;      // DBG builds: per-CTA cycle breakdown (16 counters: softmax warp 4, MMA warp)
 };
 
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (here the fp16 probabilities, lane = query row, two K elements per
-// 32-bit column) comes straight from tensor memory, so P never takes the shared-memory round trip
-__device__ __forceinline__ void tc_mma_f16_ta(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// MN-major B operand (V tile [keys][64 channels], 128-byte rows, SWIZZLE_128B): 8-key groups are SBO = 1024 B apart,
-// 64-channel column blocks are LBO apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-template <int D, int HO>   // HO: key chunk (0..7) after which a softmax warpgroup hands the MUFU pipe over
-__global__ void __launch_bounds__(ATT_THREADS, 1) attn_tc_kernel(const __grid_constant__ TAttnArgs p) {
+template <int D>
+__global__ void __launch_bounds__(ATT_THREADS) attn_tc_kernel(const __grid_constant__ TAttnArgs p) {
   using C = TCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t q_s = base;                                   // [2 tiles][NCB][128 rows x 128 B]
-  const uint32_t kv_s = q_s + C::Q_BYTES;                      // [ST][K: NCB blocks | V: NCB blocks]
-  const uint32_t p_s = kv_s + C::ST * C::KV_STAGE_BYTES;       // [2 tiles][2 buffers][128 rows x 128 B]
-  const uint32_t bars = p_s + 4 * C::P_TILE_BYTES;
+  const uint32_t q_s = base;                                   // [NCB][64 rows x 128 B]
+  const uint32_t kv_s = q_s + C::Q_BYTES;                      // [2 stages][K: NCB blocks | V: NCB blocks]
+  const uint32_t bars = kv_s + 2 * C::KV_STAGE_BYTES;
   const uint32_t q_full = bars;
   auto kv_full = [&](int s) { return bars + 8u * (1 + s); };
-  auto kv_empty = [&](int s) { return bars + 8u * (1 + C::ST + s); };
-  auto s_full = [&](int i, int b) { return bars + 8u * (1 + 2 * C::ST + 2 * i + b); };
-  auto p_full = [&](int i, int b) { return bars + 8u * (5 + 2 * C::ST + 2 * i + b); };
-  auto p_empty = [&](int i, int b) { return bars + 8u * (9 + 2 * C::ST + 2 * i + b); };
-  const uint32_t o_full = bars + 8u * (13 + 2 * C::ST);
-  auto v_ready = [&](int s) { return bars + 8u * (14 + 2 * C::ST + s); };      // ones column written into V stage s
-  const uint32_t tmem_slot = bars + 8u * (14 + 3 * C::ST);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * 2 * TQ, head = blockIdx.y, b = blockIdx.z;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, q4 = lane & 3;
+  const int q0 = blockIdx.x * TQ, head = blockIdx.y, b = blockIdx.z, bk = b / p.kv_div;
   const int nkt = (p.nk + BKV - 1) / BKV;
 
-  if (warp == 0 && lane == 0) { prefetch_tmap(&p.tmQ); prefetch_tmap(&p.tmK); prefetch_tmap(&p.tmV); }
-  if (warp == 1 && lane == 0) {
+  if (tid == 0) {
+    prefetch_tmap(&p.tmQ); prefetch_tmap(&p.tmK); prefetch_tmap(&p.tmV);
     mbar_init(q_full, 1);
-    for (int s = 0; s < C::ST; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); mbar_init(v_ready(s), 1); }
-    for (int i = 0; i < 2; ++i) {
-      for (int bb = 0; bb < 2; ++bb) {
-        mbar_init(s_full(i, bb), 1);
-        mbar_init(p_full(i, bb), 128);
-        mbar_init(p_empty(i, bb), 1);
-      }
-    }
-    mbar_init(o_full, 1);
+    mbar_init(kv_full(0), 1);
+    mbar_init(kv_full(1), 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
   pdl_trigger();
   pdl_wait();                                    // set-up above overlaps the previous kernel's tail
-
-  // Single-issuer roles run with the whole warp (uniform values) and predicate the issuing instructions on one elected
-  // lane -- see the note in gemm.cu.
-  if (warp == 0) {
-    // ================================================================ TMA producer
-    if (elect_one()) {
-      mbar_expect_tx(q_full, C::Q_BYTES);
-      for (int i = 0; i < 2; ++i)
-        for (int cb = 0; cb < C::NCB; ++cb)
-          tma_load_4d(q_s + (i * C::NCB + cb) * TQ * 128, &p.tmQ, q_full, cb * 64, head, q0 + i * TQ, b);
+  auto load_kv = [&](int j) {
+    const uint32_t s = j & 1, k_dst = kv_s + s * C::KV_STAGE_BYTES, v_dst = k_dst + C::NCB * C::BLOCK_BYTES;
+    mbar_expect_tx(kv_full(s), C::KV_STAGE_BYTES);
+#pragma unroll
+    for (int cb = 0; cb < C::NCB; ++cb) {
+      tma_load_4d(k_dst + cb * C::BLOCK_BYTES, &p.tmK, kv_full(s), cb * 64, head, j * BKV, bk);
+      tma_load_4d(v_dst + cb * C::BLOCK_BYTES, &p.tmV, kv_full(s), cb * 64, head, j * BKV, bk);
     }
-    __syncwarp();
-    const int bk = b / p.kv_div;
-    uint32_t s = 0, ph = 0;
-    for (int j = 0; j < nkt; ++j) {
-      mbar_wait(kv_empty(s), ph ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(kv_full(s), C::KV_STAGE_BYTES);
-        const uint32_t k_dst = kv_s + s * C::KV_STAGE_BYTES;
-        const uint32_t v_dst = k_dst + C::NCB * C::KV_BLOCK_BYTES;
-#pragma unroll
-        for (int cb = 0; cb < C::NCB; ++cb) {
-          tma_load_4d(k_dst + cb * C::KV_BLOCK_BYTES, &p.tmK, kv_full(s), cb * 64, head, j * BKV, bk);
-          tma_load_4d(v_dst + cb * C::KV_BLOCK_BYTES, &p.tmV, kv_full(s), cb * 64, head, j * BKV, bk);
-        }
-      }
-      __syncwarp();
-      if (++s == (uint32_t)C::ST) { s = 0; ph ^= 1; }
-    }
-  } else if (warp == 1) {
-    // ================================================================ MMA issuer
-    constexpr uint32_t idesc_qk = umma_idesc_f16(TQ, BKV);
-    constexpr uint32_t idesc_pv = umma_idesc_f16(TQ, C::DPO) | (1u << 16);   // B operand MN-major
-    auto issue_qk = [&](int i, uint32_t s, int buf) {
-      if (elect_one()) {
-        const uint32_t qa = q_s + i * C::NCB * TQ * 128;
-        const uint32_t ka = kv_s + s * C::KV_STAGE_BYTES;
-#pragma unroll
-        for (int k = 0; k < C::DPK / 16; ++k) {
-          const int cb = (k * 16) / 64, off = ((k * 16) % 64) * 2;
-          tc_mma_f16(tmem + C::S_COL + (2 * i + buf) * BKV, umma_desc_sw128_kmajor(qa + cb * TQ * 128 + off),
-                     umma_desc_sw128_kmajor(ka + cb * C::KV_BLOCK_BYTES + off), idesc_qk, k != 0 ? 1u : 0u);
-        }
-        tc_commit(s_full(i, buf));
-      }
-      __syncwarp();
-    };
-    auto issue_pv = [&](int i, uint32_t s, int pb, bool acc, bool release_kv) {
-      if (elect_one()) {
-        const uint32_t pa = p_s + (2 * i + pb) * C::P_TILE_BYTES;
-        const uint32_t va = kv_s + s * C::KV_STAGE_BYTES + C::NCB * C::KV_BLOCK_BYTES;
-#pragma unroll
-        for (int k = 0; k < BKV / 16; ++k)
-          tc_mma_f16(tmem + C::O_COL + i * C::O_STRIDE, umma_desc_sw128_kmajor(pa + k * 32),
-                     umma_desc_sw128_mnmajor(va + k * 16 * 128, C::KV_BLOCK_BYTES), idesc_pv, (acc || k != 0) ? 1u : 0u);
-        tc_commit(p_empty(i, pb));               // this P buffer consumed, O_i quiescent once this retires
-        if (release_kv) tc_commit(kv_empty(s));  // K_j / V_j fully consumed once these MMAs retire
-      }
-      __syncwarp();
-    };
-    mbar_wait(q_full, 0);
-    for (int jj = 0; jj < 2 && jj < nkt; ++jj) {     // Q K^T runs two key tiles ahead of the softmax
-      mbar_wait(kv_full(jj), 0);
-      tc_fence_after();
-      issue_qk(0, jj, jj & 1);
-      issue_qk(1, jj, jj & 1);
-    }
-    uint32_t s = 0, sph = 0;                         // stage / phase of tile j
-    uint32_t sn = 2 % C::ST, nph = (2 / C::ST) & 1;  // stage / phase of tile j + 2
-    for (int j = 0; j < nkt; ++j) {
-      const bool more = j + 2 < nkt;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        mbar_wait(p_full(i, j & 1), (j >> 1) & 1);
-        if (i == 0) mbar_wait(v_ready(s), sph);      // ones column of this V tile is in place
-        tc_fence_after();
-        issue_pv(i, s, j & 1, j > 0, i == 1);
-        if (more) {
-          if (i == 0) {
-            mbar_wait(kv_full(sn), nph);
-            tc_fence_after();
-          }
-          issue_qk(i, sn, j & 1);                    // S_{i, j&1} was drained by the softmax before it signalled p_full
-        }
-      }
-      if (++s == (uint32_t)C::ST) { s = 0; sph ^= 1; }
-      if (++sn == (uint32_t)C::ST) { sn = 0; nph ^= 1; }
-    }
-    if (elect_one()) tc_commit(o_full);
-    __syncwarp();
-  } else if (warp == 3) {
-    // ================================================================ ones column: V[:, D] = 1 for every landed V tile
-    constexpr int blk = D / 64, chunk = ((D % 64) * 2) / 16, within = ((D % 64) * 2) % 16;
-    for (int j = 0; j < nkt; ++j) {
-      const int s = j % C::ST;
-      mbar_wait(kv_full(s), (j / C::ST) & 1);
-      const uint32_t v_blk = kv_s + s * C::KV_STAGE_BYTES + (C::NCB + blk) * C::KV_BLOCK_BYTES;
-#pragma unroll
-      for (int r = lane; r < BKV; r += 32) {
-        const uint32_t dst = v_blk + r * 128 + ((chunk ^ (r & 7)) << 4) + within;
-        asm volatile("st.shared.b16 [%0], %1;" ::"r"(dst), "h"((unsigned short)0x3C00) : "memory");   // fp16 1.0
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(v_ready(s));
-    }
-  } else if (warp >= 4) {
-    // ================================================================ softmax warpgroups + epilogue
-    const int i = (warp - 4) >> 2;               // query tile handled by this warpgroup
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;         // query row inside the tile == TMEM lane
-    const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-    const uint32_t o_addr = tmem + lane_addr + C::O_COL + i * C::O_STRIDE;
-    const uint32_t p_row0 = p_s + 2 * i * C::P_TILE_BYTES + row * 128;
-    const float sc = p.scale_log2;
-    float m_used = -INFINITY;
-    // Ping-pong of the two softmax warpgroups on the MUFU pipe: a warpgroup enters its exponential phase only when the
-    // other one is (almost) through its own (256-thread named barriers 9 + i: sync = "my turn", arrive = "your turn"), so
-    // one does load / max / pack / store work while the other keeps the 16 ex2/clk/SM pipe busy.  P is double-buffered so
-    // that nothing else is on the critical path.
-    if (i == 1) named_bar_arrive(9 + 0, 256);    // warpgroup 0 goes first
-    for (int j = 0; j < nkt; ++j) {
-      mbar_wait(s_full(i, j & 1), (j >> 1) & 1);
-      tc_fence_after();
-      const int kbase = j * BKV;
-      // ---- the S row of this tile lives in registers: one TMEM round trip per tile
-      uint32_t sv[BKV];
-      const uint32_t s_addr = tmem + lane_addr + C::S_COL + (2 * i + (j & 1)) * BKV;
-      tmem_ld32(s_addr, sv);
-      tmem_ld32(s_addr + 32, sv + 32);
-      tmem_ld_wait();
-      if (kbase + BKV > p.nk) {   // keys beyond nk were zero-filled by TMA: mask them (last tile only)
-#pragma unroll
-        for (int t = 0; t < BKV; ++t)
-          if (kbase + t >= p.nk) sv[t] = 0xff800000u;   // -inf
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-      for (int t = 0; t < BKV; t += 8) {           // FMNMX3: two new elements per instruction, four independent chains
-        mx0 = fmax3(mx0, __uint_as_float(sv[t]), __uint_as_float(sv[t + 1]));
-        mx1 = fmax3(mx1, __uint_as_float(sv[t + 2]), __uint_as_float(sv[t + 3]));
-        mx2 = fmax3(mx2, __uint_as_float(sv[t + 4]), __uint_as_float(sv[t + 5]));
-        mx3 = fmax3(mx3, __uint_as_float(sv[t + 6]), __uint_as_float(sv[t + 7]));
-      }
-      const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      // ---- lazy rescale: only when the maximum moved by more than 2^8 (always true on the first tile: m_used=-inf)
-      const bool need = (mx - m_used) * sc > 8.f;
-      if (j > 0 && __any_sync(0xffffffffu, need)) {
-        mbar_wait(p_empty(i, (j - 1) & 1), ((j - 1) >> 1) & 1);       // O_i quiescent: the previous P V has retired
-        tc_fence_after();
-        const float alpha = need ? exp2f((m_used - mx) * sc) : 1.f;   // also rescales the row-sum column O[:, D]
-#pragma unroll 1
-        for (int c0 = 0; c0 < C::DPO; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld16(o_addr + c0, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int t = 0; t < 16; ++t) v[t] = __float_as_uint(__uint_as_float(v[t]) * alpha);
-          tmem_st16(o_addr + c0, v);
-        }
-        tmem_st_wait();
-      }
-      if (need) m_used = mx;
-      const float ms = m_used * sc;
-      if (j >= 2) mbar_wait(p_empty(i, j & 1), ((j - 2) >> 1) & 1);   // this P buffer was consumed two key tiles ago
-      const uint32_t p_row = p_row0 + (j & 1) * C::P_TILE_BYTES;
-      named_bar_sync(9 + i, 256);                                       // my turn on the MUFU pipe
-      // ---- P = exp2(S*scale - m) -> fp16 -> swizzled shared memory (A operand of the P V MMA); exp2(-inf) = 0 masks
-#pragma unroll
-      for (int c8 = 0; c8 < BKV / 8; ++c8) {       // one 16-byte chunk (8 keys) at a time
-        uint32_t pk[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const float e0 = fast_exp2(__uint_as_float(sv[c8 * 8 + 2 * u]) * sc - ms);
-          const float e1 = fast_exp2(__uint_as_float(sv[c8 * 8 + 2 * u + 1]) * sc - ms);
-          const __half2 h = __floats2half2_rn(e0, e1);   // the row sum is formed by the MMA from these rounded values
-          pk[u] = *reinterpret_cast<const uint32_t*>(&h);
-        }
-        const uint32_t dst = p_row + ((c8 ^ (row & 7)) << 4);
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3])
-                     : "memory");
-        // hand the MUFU pipe to the other warpgroup a little before the last exponentials (its wake-up takes a while)
-        if (c8 == HO) named_bar_arrive(9 + (i ^ 1), 256);
-      }
-      fence_proxy_async();                     // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-      tc_fence_before();
-      mbar_arrive(p_full(i, j & 1));
-    }
-    if (i == 0) named_bar_sync(9 + 0, 256);      // absorb the other warpgroup's last hand-over
-    // ---- epilogue: O / l -> fp16 -> HBM
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const int qrow = q0 + i * TQ + row;
-    float inv;
-    {   // softmax denominator = the ones column of the accumulator
-      uint32_t v[16];
-      tmem_ld16(o_addr + (D / 16) * 16, v);
-      tmem_ld_wait();
-      inv = 1.f / __uint_as_float(v[D % 16]);
-    }
-    __half* orow = p.o + b * p.o_bs + (long long)qrow * p.ldo + head * D;
-#pragma unroll 1
-    for (int c0 = 0; c0 < C::DPO; c0 += 16) {
-      uint32_t v[16];
-      tmem_ld16(o_addr + c0, v);
-      tmem_ld_wait();
-      if (qrow < p.nq) {
-#pragma unroll
-        for (int t = 0; t < 16; t += 8) {
-          if (c0 + t < D) {
-            uint4 o4;
-            __half2* h = reinterpret_cast<__half2*>(&o4);
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-              h[u] = __floats2half2_rn(__uint_as_float(v[t + 2 * u]) * inv, __uint_as_float(v[t + 2 * u + 1]) * inv);
-            *reinterpret_cast<uint4*>(orow + c0 + t) = o4;
-          }
-        }
-      }
-    }
+  };
+  if (tid == 0) {
+    mbar_expect_tx(q_full, C::Q_BYTES);
+    for (int cb = 0; cb < C::NCB; ++cb) tma_load_4d(q_s + cb * C::BLOCK_BYTES, &p.tmQ, q_full, cb * 64, head, q0, b);
+    load_kv(0);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::TMEM_COLS);
+
+  const float sc = p.scale_log2;
+  float o[C::OREG];
+#pragma unroll
+  for (int i = 0; i < C::OREG; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};      // rows lane / 4 and lane / 4 + 8 of this warp
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nkt; ++j) {
+    // every warp is past tile j - 1, so its stage may be refilled with tile j + 1 while tile j is computed
+    __syncthreads();
+    if (tid == 0 && j + 1 < nkt) load_kv(j + 1);
+    mbar_wait(kv_full(j & 1), (j >> 1) & 1);
+    const uint32_t k_a = kv_s + (j & 1) * C::KV_STAGE_BYTES, v_a = k_a + C::NCB * C::BLOCK_BYTES;
+    // ---- S = Q K^T
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < C::DPK / 16; ++k) {
+      const uint32_t off = (uint32_t)((k * 16) / 64) * C::BLOCK_BYTES + (uint32_t)((k * 16) % 64) * 2;
+      wgmma_m64n64(s, gmma_desc_sw128(q_s + off), gmma_desc_sw128(k_a + off), k != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    const int kbase = j * BKV;
+    if (kbase + BKV > p.nk) {                    // keys beyond nk (last tile only)
+#pragma unroll
+      for (int i = 0; i < 32; ++i)
+        if (kbase + 8 * (i >> 2) + 2 * q4 + (i & 1) >= p.nk) s[i] = -INFINITY;
+    }
+    // ---- online softmax (row h = 0: registers with (i >> 1) even, h = 1: odd)
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = m[h];
+#pragma unroll
+      for (int i = 2 * h; i < 32; i += 4) mx = fmaxf(mx, fmaxf(s[i], s[i + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      alpha[h] = fast_exp2((m[h] - mx) * sc);    // exp2(-inf) = 0 on the first tile
+      m[h] = mx;
+      const float ms = mx * sc;
+      float rs = 0.f;
+#pragma unroll
+      for (int i = 2 * h; i < 32; i += 4) {
+        s[i] = fast_exp2(fmaf(s[i], sc, -ms));
+        s[i + 1] = fast_exp2(fmaf(s[i + 1], sc, -ms));
+        rs += s[i] + s[i + 1];
+      }
+      l[h] = fmaf(l[h], alpha[h], rs);
+    }
+#pragma unroll
+    for (int i = 0; i < C::OREG; ++i) o[i] *= alpha[(i >> 1) & 1];
+    // ---- O += P V: P (fp16) as the register A operand, 16 keys per instruction.  All of P is packed before the fence,
+    // so no register the wgmmas read is written between them.
+    uint32_t a[BKV / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk)
+#pragma unroll
+      for (int r = 0; r < 4; ++r) a[kk][r] = pack_h2(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) {
+      const uint32_t v_rows = v_a + kk * 16 * 128;
+      wgmma_m64n64_rs<1>(o, a[kk], gmma_desc_sw128_mn(v_rows, C::BLOCK_BYTES), 1u);
+      if (D > 64) wgmma_m64n16_rs<1>(o + 32, a[kk], gmma_desc_sw128_mn(v_rows + C::BLOCK_BYTES, C::BLOCK_BYTES), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+  }
+  // ---- epilogue: O / l -> fp16 -> HBM
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 1);
+    l[h] += __shfl_xor_sync(0xffffffffu, l[h], 2);
+  }
+  const float inv[2] = {1.f / l[0], 1.f / l[1]};
+  const int r0 = q0 + 16 * warp + (lane >> 2);
+  __half* ob = p.o + b * p.o_bs + head * D;
+#pragma unroll
+  for (int i = 0; i < C::OREG; i += 2) {
+    const int h = (i >> 1) & 1, c = 8 * (i >> 2) + 2 * q4, r = r0 + 8 * h;
+    if (c < D && r < p.nq)
+      *reinterpret_cast<__half2*>(ob + (long long)r * p.ldo + c) = __floats2half2_rn(o[i] * inv[h], o[i + 1] * inv[h]);
   }
 }
 
-// exp2 on the FMA pipe (Cody-Waite split + cubic minimax of 2^f on [-0.5, 0.5], |rel err| <= 7.5e-5 -- below the fp16
-// rounding of P): the softmax of d = 40 attention needs 16 384 exponentials per 128 x 128 score tile against ~200 tensor
-// cycles, so the 16/clk/SM MUFU pipe is the bound; a share of the exponentials is moved onto the (idle) FMA pipe.
-__device__ __forceinline__ float exp2_fma(float x) {
-  x = fmaxf(x, -126.f);
-  const float t = x + 12582912.f;                  // 1.5 * 2^23: round(x) lands in the low mantissa bits
-  const float f = x - (t - 12582912.f);
-  float pl = fmaf(f, 0.05517166f, 0.24261112f);
-  pl = fmaf(pl, f, 0.69326099f);
-  pl = fmaf(pl, f, 0.99992807f);
-  return __int_as_float(__float_as_int(pl) + (__float_as_int(t) << 23));   // * 2^round(x) through the exponent field
-}
-
-// PERSISTENT variant (default): one CTA per SM walks work items (batch, head, 256-query block) round-robin.  Every role
-// keeps running counters across items, so the K/V ring, the S / P double buffers and the MUFU ping-pong never drain at
-// an item boundary: the producer prefetches the next item's Q (double-buffered for d <= 64) and first K/V tiles while
-// the current item finishes, Q K^T of the next item is issued two key tiles ahead as inside an item, and a softmax
-// warpgroup writes its O tile out while the other one keeps the MUFU pipe busy.  This removes the per-CTA prologue
-// (barrier init, TMEM allocation, Q + first K/V round trip: 15 % of the softmax warps' time at N = 4096 and nearly all
-// of it for the 2-tile cross-attention CTAs) and the wave tail.  O needs no double buffering: P V of item n+1 / tile i
-// is only issued after p_full(i), which warpgroup i signals after its epilogue of item n.
-// NPOLY of the 8 sixteen-byte P chunks per key tile take their exponentials from exp2_fma instead of MUFU.EX2.
-// EPIWG (d <= 64, where TMEM has room for a second pair of O accumulators): a fourth warpgroup (warps 12-15) writes the
-// finished O tiles out, so the two softmax warpgroups run one uninterrupted stream of key tiles -- with the epilogue
-// inside the softmax warpgroups the strict MUFU ping-pong stalls both of them at every item boundary.
-template <int D, int HO, int NPOLY, bool EPIWG, bool DBG, bool PP = true, bool PTMEM = false>
-__global__ void __launch_bounds__(EPIWG ? ATT_THREADS + 128 : ATT_THREADS, 1) attn_tcp_kernel(const __grid_constant__ TAttnArgs p) {
-  using C = TCfg<D>;
-  static_assert(!EPIWG || C::O_COL + 4 * C::O_STRIDE <= 512, "no TMEM room for double-buffered O");
-  constexpr int QB = (D <= 64) ? 2 : 1;                        // Q buffers
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t q_s = base;                                   // [QB][2 tiles][NCB][128 rows x 128 B]
-  const uint32_t kv_s = q_s + QB * C::Q_BYTES;                 // [ST][K: NCB blocks | V: NCB blocks]
-  const uint32_t p_s = kv_s + C::ST * C::KV_STAGE_BYTES;       // [2 tiles][2 buffers][128 rows x 128 B]
-  const uint32_t bars = p_s + 4 * C::P_TILE_BYTES;
-  auto q_full = [&](int b) { return bars + 8u * b; };
-  auto q_empty = [&](int b) { return bars + 8u * (2 + b); };
-  auto kv_full = [&](int s) { return bars + 8u * (4 + s); };
-  auto kv_empty = [&](int s) { return bars + 8u * (4 + C::ST + s); };
-  auto v_ready = [&](int s) { return bars + 8u * (4 + 2 * C::ST + s); };
-  auto s_full = [&](int i, int b) { return bars + 8u * (4 + 3 * C::ST + 2 * i + b); };
-  auto p_full = [&](int i, int b) { return bars + 8u * (8 + 3 * C::ST + 2 * i + b); };
-  auto p_empty = [&](int i, int b) { return bars + 8u * (12 + 3 * C::ST + 2 * i + b); };
-  auto o_full = [&](int i, int ob) { return bars + 8u * (16 + 3 * C::ST + 2 * i + ob); };    // per (tile, O buffer)
-  auto o_empty = [&](int i, int ob) { return bars + 8u * (20 + 3 * C::ST + 2 * i + ob); };
-  const uint32_t tmem_slot = bars + 8u * (24 + 3 * C::ST);
-  auto o_col = [&](int i, uint32_t n) { return (uint32_t)(C::O_COL + (EPIWG ? ((n & 1) * 2 + i) : i) * C::O_STRIDE); };
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkt = (p.nk + BKV - 1) / BKV;
-  const int item0 = blockIdx.x, istep = gridDim.x;
-
-  if (warp == 0 && lane == 0) { prefetch_tmap(&p.tmQ); prefetch_tmap(&p.tmK); prefetch_tmap(&p.tmV); }
-  if (warp == 1 && lane == 0) {
-    for (int b = 0; b < 2; ++b) { mbar_init(q_full(b), 1); mbar_init(q_empty(b), 1); }
-    for (int s = 0; s < C::ST; ++s) { mbar_init(kv_full(s), 1); mbar_init(kv_empty(s), 1); mbar_init(v_ready(s), 1); }
-    for (int i = 0; i < 2; ++i) {
-      for (int bb = 0; bb < 2; ++bb) {
-        mbar_init(s_full(i, bb), 1);
-        mbar_init(p_full(i, bb), 128);
-        mbar_init(p_empty(i, bb), 1);
-        mbar_init(o_full(i, bb), 1);
-        mbar_init(o_empty(i, bb), 128);
-      }
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_slot, C::TMEM_COLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot_ptr;
-  pdl_trigger();
-  pdl_wait();                                    // set-up above overlaps the previous kernel's tail
-
-  if (warp == 0) {
-    // ================================================================ TMA producer
-    uint32_t g = 0, n = 0;                       // running key-tile / item counters
-    for (int item = item0; item < p.n_items; item += istep, ++n) {
-      const int qblk = item % p.n_qblk, bh = item / p.n_qblk, head = bh % p.heads, b = bh / p.heads;
-      const int q0 = qblk * 2 * TQ, bk = b / p.kv_div;
-      const uint32_t qb = n % QB;
-      if (n >= (uint32_t)QB) mbar_wait(q_empty(qb), ((n / QB) - 1) & 1);    // the item that used this Q buffer issued its last Q K^T
-      if (elect_one()) {
-        mbar_expect_tx(q_full(qb), C::Q_BYTES);
-        for (int i = 0; i < 2; ++i)
-          for (int cb = 0; cb < C::NCB; ++cb)
-            tma_load_4d(q_s + qb * C::Q_BYTES + (i * C::NCB + cb) * TQ * 128, &p.tmQ, q_full(qb), cb * 64, head, q0 + i * TQ, b);
-      }
-      __syncwarp();
-      for (int j = 0; j < nkt; ++j, ++g) {
-        const uint32_t s = g % C::ST;
-        mbar_wait(kv_empty(s), ((g / C::ST) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_expect_tx(kv_full(s), C::KV_STAGE_BYTES);
-          const uint32_t k_dst = kv_s + s * C::KV_STAGE_BYTES;
-          const uint32_t v_dst = k_dst + C::NCB * C::KV_BLOCK_BYTES;
-#pragma unroll
-          for (int cb = 0; cb < C::NCB; ++cb) {
-            tma_load_4d(k_dst + cb * C::KV_BLOCK_BYTES, &p.tmK, kv_full(s), cb * 64, head, j * BKV, bk);
-            tma_load_4d(v_dst + cb * C::KV_BLOCK_BYTES, &p.tmV, kv_full(s), cb * 64, head, j * BKV, bk);
-          }
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    // ================================================================ P V issuer
-    // The tcgen05.mma issue path of ONE warp (descriptor set-up in uniform registers, ~7 MMAs + 3 commits + 3-4 mbarrier
-    // polls per key tile and query tile) measured ~700 clk per round with the softmax warps waiting ~530 clk per tile for
-    // S (profiles/r02_attn_debug_counters.json): the single issuer, not the MUFU pipe, bounded the steady state.  The two
-    // GEMMs are therefore issued by two warps: this one issues O_i += P_i V, warp 2 issues S_i = Q_i K^T.
-    constexpr uint32_t idesc_pv = umma_idesc_f16(TQ, C::DPO) | (1u << 16);   // B operand MN-major
-    const int my_items = (p.n_items - item0 + istep - 1) / istep;
-    const uint32_t total = (uint32_t)my_items * (uint32_t)nkt;               // key tiles this CTA walks
-    long long m_p0 = 0, m_p1 = 0, m_v = 0, m_oe = 0, m_t0 = 0;
-    const bool mdbg = DBG && lane == 0 && p.dbg != nullptr;
-#define VS_MT() (mdbg ? clock64() : 0LL)
-    if (DBG) m_t0 = VS_MT();
-    int j = 0;
-    uint32_t n = 0;                                  // item of the P V cursor
-    for (uint32_t g = 0; g < total; ++g) {
-      const uint32_t s = g % C::ST, sph = (g / C::ST) & 1;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        long long ta = 0;
-        if (DBG) ta = VS_MT();
-        mbar_wait(p_full(i, g & 1), (g >> 1) & 1);
-        if (DBG) { const long long tb = VS_MT(); if (i == 0) m_p0 += tb - ta; else m_p1 += tb - ta; ta = tb; }
-        if (i == 0) mbar_wait(v_ready(s), sph);      // ones column of this V tile is in place
-        if (DBG) { const long long tb = VS_MT(); m_v += tb - ta; ta = tb; }
-        if (EPIWG && j == 0 && n >= 2) mbar_wait(o_empty(i, n & 1), ((n >> 1) - 1) & 1);   // the epilogue warps drained this O buffer
-        if (DBG) m_oe += VS_MT() - ta;
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t pa = p_s + (2 * i + (g & 1)) * C::P_TILE_BYTES;
-          const uint32_t va = kv_s + s * C::KV_STAGE_BYTES + C::NCB * C::KV_BLOCK_BYTES;
-#pragma unroll
-          for (int k = 0; k < BKV / 16; ++k) {
-            if (PTMEM)      // P_{i, g&1} lives in the first 32 columns of the S buffer it was computed from (8 columns per k16)
-              tc_mma_f16_ta(tmem + o_col(i, n), tmem + C::S_COL + (2 * i + (g & 1)) * BKV + k * 8,
-                            umma_desc_sw128_mnmajor(va + k * 16 * 128, C::KV_BLOCK_BYTES), idesc_pv, (j > 0 || k != 0) ? 1u : 0u);
-            else
-              tc_mma_f16(tmem + o_col(i, n), umma_desc_sw128_kmajor(pa + k * 32),
-                         umma_desc_sw128_mnmajor(va + k * 16 * 128, C::KV_BLOCK_BYTES), idesc_pv, (j > 0 || k != 0) ? 1u : 0u);
-          }
-          tc_commit(p_empty(i, g & 1));              // this P buffer consumed, O_i quiescent once this retires
-          if (i == 1) tc_commit(kv_empty(s));        // V_j consumed (K_j was consumed by Q K^T of this tile, long retired)
-          if (j == nkt - 1) tc_commit(o_full(i, EPIWG ? (n & 1) : 0));   // O_i of this item complete
-        }
-        __syncwarp();
-      }
-      if (++j == nkt) { j = 0; ++n; }
-    }
-    if (mdbg) {
-      unsigned long long* d = p.dbg + 16 * blockIdx.x + 8;
-      d[0] = (unsigned long long)(clock64() - m_t0); d[3] = m_p0; d[4] = m_p1; d[5] = m_v; d[6] = m_oe;
-    }
-#undef VS_MT
-  } else if (warp == 2) {
-    // ================================================================ Q K^T issuer (after the TMEM allocation above)
-    // Runs two key tiles ahead of the softmax, across item boundaries: S_{i, g&1} of tile g may be overwritten once the
-    // softmax of tile g-2 has drained it, which it signals with p_full(i, (g-2)&1) (also awaited by the P V issuer).
-    constexpr uint32_t idesc_qk = umma_idesc_f16(TQ, BKV);
-    const int my_items = (p.n_items - item0 + istep - 1) / istep;
-    const uint32_t total = (uint32_t)my_items * (uint32_t)nkt;
-    long long m_q = 0, m_kv = 0, m_pf = 0;
-    const bool mdbg = DBG && lane == 0 && p.dbg != nullptr;
-#define VS_MT() (mdbg ? clock64() : 0LL)
-    uint32_t nq_item = 0; int jq = 0;
-    for (uint32_t gq = 0; gq < total; ++gq) {
-      const uint32_t s = gq % C::ST, qb = nq_item % QB;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        long long ta = 0;
-        if (DBG) ta = VS_MT();
-        // S_{i, gq&1} is free once the softmax of tile gq-2 drained it (p_full) -- or, when P lives in that same TMEM region
-        // (PTMEM), once P V of tile gq-2 has consumed it (p_empty)
-        if (gq >= 2) mbar_wait(PTMEM ? p_empty(i, gq & 1) : p_full(i, gq & 1), ((gq - 2) >> 1) & 1);
-        if (DBG) { const long long tb = VS_MT(); m_pf += tb - ta; ta = tb; }
-        if (i == 0) {
-          if (jq == 0) mbar_wait(q_full(qb), (nq_item / QB) & 1);
-          if (DBG) { const long long tb = VS_MT(); m_q += tb - ta; ta = tb; }
-          mbar_wait(kv_full(s), (gq / C::ST) & 1);
-          if (DBG) m_kv += VS_MT() - ta;
-        }
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t qa = q_s + qb * C::Q_BYTES + i * C::NCB * TQ * 128;
-          const uint32_t ka = kv_s + s * C::KV_STAGE_BYTES;
-#pragma unroll
-          for (int k = 0; k < C::DPK / 16; ++k) {
-            const int cb = (k * 16) / 64, off = ((k * 16) % 64) * 2;
-            tc_mma_f16(tmem + C::S_COL + (2 * i + (gq & 1)) * BKV, umma_desc_sw128_kmajor(qa + cb * TQ * 128 + off),
-                       umma_desc_sw128_kmajor(ka + cb * C::KV_BLOCK_BYTES + off), idesc_qk, k != 0 ? 1u : 0u);
-          }
-          tc_commit(s_full(i, gq & 1));
-          if (i == 1 && jq == nkt - 1) tc_commit(q_empty(qb));     // last Q K^T of this item: its Q buffer may be refilled
-        }
-        __syncwarp();
-      }
-      if (++jq == nkt) { jq = 0; ++nq_item; }
-    }
-    if (mdbg) {
-      unsigned long long* d = p.dbg + 16 * blockIdx.x + 8;
-      d[1] = m_q; d[2] = m_kv; d[7] = m_pf;          // slots 0, 3..6 belong to the P V issuer; 7 = wait for a free S buffer
-    }
-#undef VS_MT
-  } else if (warp == 3) {
-    // ================================================================ ones column: V[:, D] = 1 for every landed V tile
-    constexpr int blk = D / 64, chunk = ((D % 64) * 2) / 16, within = ((D % 64) * 2) % 16;
-    const int my_items = (p.n_items - item0 + istep - 1) / istep;
-    const uint32_t total = (uint32_t)my_items * (uint32_t)nkt;
-    for (uint32_t g = 0; g < total; ++g) {
-      const uint32_t s = g % C::ST;
-      mbar_wait(kv_full(s), (g / C::ST) & 1);
-      const uint32_t v_blk = kv_s + s * C::KV_STAGE_BYTES + (C::NCB + blk) * C::KV_BLOCK_BYTES;
-#pragma unroll
-      for (int r = lane; r < BKV; r += 32) {
-        const uint32_t dst = v_blk + r * 128 + ((chunk ^ (r & 7)) << 4) + within;
-        asm volatile("st.shared.b16 [%0], %1;" ::"r"(dst), "h"((unsigned short)0x3C00) : "memory");   // fp16 1.0
-      }
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(v_ready(s));
-    }
-  } else if (warp >= 4 && warp < 12) {
-    // ================================================================ softmax warpgroups (+ epilogue unless EPIWG)
-    const int i = (warp - 4) >> 2;               // query tile handled by this warpgroup
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;         // query row inside the tile == TMEM lane
-    const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-    const uint32_t p_row0 = p_s + 2 * i * C::P_TILE_BYTES + row * 128;
-    const float sc = p.scale_log2;
-    // DBG: cycle breakdown seen by lane 0 of warp 4: [0] total [1] wait S [2] wait turn [3] wait P buffer / rescale
-    // [4] exponential phase [5] epilogue [6] items [7] key tiles
-    long long t_ws = 0, t_ws0 = 0, t_wt = 0, t_wp = 0, t_ex = 0, t_ep = 0, t0 = 0, tt = 0;
-    const bool dbg = DBG && warp == 4 && lane == 0 && p.dbg != nullptr;
-#define VS_TICK() (dbg ? clock64() : 0LL)
-    if (DBG) t0 = VS_TICK();
-    if (PP && i == 1) named_bar_arrive(9 + 0, 256);    // warpgroup 0 goes first on the MUFU pipe
-    uint32_t g = 0, n = 0;
-    for (int item = item0; item < p.n_items; item += istep, ++n) {
-      const int qblk = item % p.n_qblk, bh = item / p.n_qblk, head = bh % p.heads, b = bh / p.heads;
-      const uint32_t o_addr = tmem + lane_addr + o_col(i, n);
-      float m_used = -INFINITY;
-      for (int j = 0; j < nkt; ++j, ++g) {
-        if (DBG) tt = VS_TICK();
-        mbar_wait(s_full(i, g & 1), (g >> 1) & 1);
-        if (DBG) { const long long dt = VS_TICK() - tt; if (j == 0) t_ws0 += dt; else t_ws += dt; }
-        tc_fence_after();
-        const int kbase = j * BKV;
-        uint32_t sv[BKV];
-        const uint32_t s_addr = tmem + lane_addr + C::S_COL + (2 * i + (g & 1)) * BKV;
-        tmem_ld32(s_addr, sv);
-        tmem_ld32(s_addr + 32, sv + 32);
-        tmem_ld_wait();
-        if (kbase + BKV > p.nk) {   // keys beyond nk were zero-filled by TMA: mask them (last tile only)
-#pragma unroll
-          for (int t = 0; t < BKV; ++t)
-            if (kbase + t >= p.nk) sv[t] = 0xff800000u;   // -inf
-        }
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-        for (int t = 0; t < BKV; t += 8) {
-          mx0 = fmax3(mx0, __uint_as_float(sv[t]), __uint_as_float(sv[t + 1]));
-          mx1 = fmax3(mx1, __uint_as_float(sv[t + 2]), __uint_as_float(sv[t + 3]));
-          mx2 = fmax3(mx2, __uint_as_float(sv[t + 4]), __uint_as_float(sv[t + 5]));
-          mx3 = fmax3(mx3, __uint_as_float(sv[t + 6]), __uint_as_float(sv[t + 7]));
-        }
-        const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-        // lazy rescale: only when the maximum moved by more than 2^8 (always "needed" on the first tile: m_used = -inf,
-        // but there O is overwritten by the non-accumulating P V, so nothing is rescaled)
-        const bool need = (mx - m_used) * sc > 8.f;
-        if (DBG) tt = VS_TICK();
-        if (j > 0 && __any_sync(0xffffffffu, need)) {
-          mbar_wait(p_empty(i, (g - 1) & 1), ((g - 1) >> 1) & 1);       // O_i quiescent: the previous P V has retired
-          tc_fence_after();
-          const float alpha = need ? exp2f((m_used - mx) * sc) : 1.f;   // also rescales the row-sum column O[:, D]
-#pragma unroll 1
-          for (int c0 = 0; c0 < C::DPO; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(o_addr + c0, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int t = 0; t < 16; ++t) v[t] = __float_as_uint(__uint_as_float(v[t]) * alpha);
-            tmem_st16(o_addr + c0, v);
-          }
-          tmem_st_wait();
-        }
-        if (need) m_used = mx;
-        const float ms = m_used * sc;
-        if (!PTMEM && g >= 2) mbar_wait(p_empty(i, g & 1), ((g - 2) >> 1) & 1);   // this P buffer was consumed two key tiles ago
-        // (PTMEM: P aliases the S buffer just read; Q K^T of this tile already waited for P V of tile g-2)
-        if (DBG) { const long long t = VS_TICK(); t_wp += t - tt; tt = t; }
-        const uint32_t p_row = p_row0 + (g & 1) * C::P_TILE_BYTES;
-        if (PP) named_bar_sync(9 + i, 256);                               // my turn on the MUFU pipe
-        if (DBG) { const long long t = VS_TICK(); t_wt += t - tt; tt = t; }
-        uint32_t pt[16];
-#pragma unroll
-        for (int c8 = 0; c8 < BKV / 8; ++c8) {       // one 16-byte chunk (8 keys) at a time
-          // chunks spread evenly over the tile take the FMA-pipe exponential (NPOLY of 8)
-          const bool poly = ((c8 + 1) * NPOLY) / 8 > (c8 * NPOLY) / 8;      // compile-time after unrolling
-          uint32_t pk[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const float x0 = __uint_as_float(sv[c8 * 8 + 2 * u]) * sc - ms, x1 = __uint_as_float(sv[c8 * 8 + 2 * u + 1]) * sc - ms;
-            const float e0 = poly ? exp2_fma(x0) : fast_exp2(x0);
-            const float e1 = poly ? exp2_fma(x1) : fast_exp2(x1);
-            const __half2 h = __floats2half2_rn(e0, e1);   // the row sum is formed by the MMA from these rounded values
-            pk[u] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-          if (PTMEM) {                           // P -> TMEM (fp16 pairs, 4 columns per chunk), 16 columns per store
-            pt[(c8 & 3) * 4 + 0] = pk[0]; pt[(c8 & 3) * 4 + 1] = pk[1]; pt[(c8 & 3) * 4 + 2] = pk[2]; pt[(c8 & 3) * 4 + 3] = pk[3];
-            if ((c8 & 3) == 3) tmem_st16(s_addr + (c8 >> 2) * 16, pt);
-          } else {
-            const uint32_t dst = p_row + ((c8 ^ (row & 7)) << 4);
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pk[0]), "r"(pk[1]), "r"(pk[2]), "r"(pk[3])
-                         : "memory");
-          }
-          if (PP && c8 == HO) named_bar_arrive(9 + (i ^ 1), 256);   // hand the MUFU pipe over a little early (wake-up latency)
-        }
-        if (PTMEM) tmem_st_wait();               // P is in tensor memory: no shared-memory round trip, no proxy fence
-        else fence_proxy_async();                // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-        tc_fence_before();
-        mbar_arrive(p_full(i, g & 1));
-        if (DBG) t_ex += VS_TICK() - tt;
-      }
-      if (EPIWG) continue;                       // warps 12-15 write O out
-      // ---- epilogue of this item: O / l -> fp16 -> HBM
-      if (DBG) tt = VS_TICK();
-      mbar_wait(o_full(i, 0), n & 1);
-      tc_fence_after();
-      const int qrow = qblk * 2 * TQ + i * TQ + row;
-      float inv;
-      {   // softmax denominator = the ones column of the accumulator
-        uint32_t v[16];
-        tmem_ld16(o_addr + (D / 16) * 16, v);
-        tmem_ld_wait();
-        inv = 1.f / __uint_as_float(v[D % 16]);
-      }
-      __half* orow = p.o + b * p.o_bs + (long long)qrow * p.ldo + head * D;
-#pragma unroll 1
-      for (int c0 = 0; c0 < C::DPO; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld16(o_addr + c0, v);
-        tmem_ld_wait();
-        if (qrow < p.nq) {
-#pragma unroll
-          for (int t = 0; t < 16; t += 8) {
-            if (c0 + t < D) {
-              uint4 o4;
-              __half2* h = reinterpret_cast<__half2*>(&o4);
-#pragma unroll
-              for (int u = 0; u < 4; ++u)
-                h[u] = __floats2half2_rn(__uint_as_float(v[t + 2 * u]) * inv, __uint_as_float(v[t + 2 * u + 1]) * inv);
-              *reinterpret_cast<uint4*>(orow + c0 + t) = o4;
-            }
-          }
-        }
-      }
-      tc_fence_before();                         // the O reads above are ordered before this warpgroup's next p_full arrive
-      if (DBG) t_ep += VS_TICK() - tt;
-    }
-    if (PP && i == 0) named_bar_sync(9 + 0, 256);      // absorb the other warpgroup's last hand-over
-    if (dbg) {
-      unsigned long long* d = p.dbg + 16 * blockIdx.x;
-      d[0] = (unsigned long long)(clock64() - t0); d[1] = t_ws; d[2] = t_wt; d[3] = t_wp; d[4] = t_ex; d[5] = t_ep; d[6] = t_ws0; d[7] = g;
-    }
-#undef VS_TICK
-  } else if (EPIWG && warp >= 12) {
-    // ================================================================ epilogue warpgroup: O / l -> fp16 -> HBM
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(quarter * 32) << 16;
-    uint32_t n = 0;
-    for (int item = item0; item < p.n_items; item += istep, ++n) {
-      const int qblk = item % p.n_qblk, bh = item / p.n_qblk, head = bh % p.heads, b = bh / p.heads;
-#pragma unroll 1
-      for (int i = 0; i < 2; ++i) {
-        mbar_wait(o_full(i, n & 1), (n >> 1) & 1);
-        tc_fence_after();
-        const uint32_t o_addr = tmem + lane_addr + o_col(i, n);
-        const int qrow = qblk * 2 * TQ + i * TQ + row;
-        float inv;
-        {
-          uint32_t v[16];
-          tmem_ld16(o_addr + (D / 16) * 16, v);
-          tmem_ld_wait();
-          inv = 1.f / __uint_as_float(v[D % 16]);
-        }
-        __half* orow = p.o + b * p.o_bs + (long long)qrow * p.ldo + head * D;
-#pragma unroll 1
-        for (int c0 = 0; c0 < C::DPO; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld16(o_addr + c0, v);
-          tmem_ld_wait();
-          if (qrow < p.nq) {
-#pragma unroll
-            for (int t = 0; t < 16; t += 8) {
-              if (c0 + t < D) {
-                uint4 o4;
-                __half2* h = reinterpret_cast<__half2*>(&o4);
-#pragma unroll
-                for (int u = 0; u < 4; ++u)
-                  h[u] = __floats2half2_rn(__uint_as_float(v[t + 2 * u]) * inv, __uint_as_float(v[t + 2 * u + 1]) * inv);
-                *reinterpret_cast<uint4*>(orow + c0 + t) = o4;
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(o_empty(i, n & 1));          // this O buffer may be overwritten by the item after next
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::TMEM_COLS);
-  }
-}
-
-unsigned long long* g_attn_dbg = nullptr;     // 148 x 8 counters (DBG kernels), see vs_debug_read
-
-template <int D, int HO, int NPOLY, bool PERSIST, bool EPIWG = false, bool DBG = false, bool PP = true, bool PTMEM = false>
+template <int D>
 int launch(cudaStream_t st, const __half* q, int ldq, const __half* k, int ldk, const __half* v, int ldv, __half* o, int ldo,
            int batch, int nq, int nk, int heads, long long q_bs, long long kv_bs, long long o_bs, int kv_div) {
   using C = TCfg<D>;
-  constexpr int SMEM_P = C::SMEM + ((D <= 64) ? C::Q_BYTES : 0) + 128;     // persistent: second Q buffer, more barriers
-  static_assert(SMEM_P <= 227 * 1024, "shared memory budget (persistent)");
   static bool configured = false;
   if (!configured) {
-    if constexpr (PERSIST) VS_CHECK_CUDA(cudaFuncSetAttribute(attn_tcp_kernel<D, HO, NPOLY, EPIWG, DBG, PP, PTMEM>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_P));
-    else VS_CHECK_CUDA(cudaFuncSetAttribute(attn_tc_kernel<D, HO>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+    VS_CHECK_CUDA(cudaFuncSetAttribute(attn_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
     configured = true;
   }
   TAttnArgs a;
@@ -834,84 +205,21 @@ int launch(cudaStream_t st, const __half* q, int ldq, const __half* k, int ldk, 
   }
   a.o = o; a.ldo = ldo; a.o_bs = o_bs; a.nq = nq; a.nk = nk; a.kv_div = kv_div;
   a.scale_log2 = 1.4426950408889634f / sqrtf((float)D);
-  a.heads = heads;
-  a.n_qblk = (nq + 2 * TQ - 1) / (2 * TQ);
-  a.n_items = a.n_qblk * heads * batch;
   ProfScope prof(st, PC_ATTN, 4.0 * batch * heads * (double)nq * nk * D, 1, nq, nk, D);
-  if constexpr (PERSIST) {
-    const int ctas = a.n_items < num_sms() ? a.n_items : num_sms();
-    if (DBG) {
-      if (!g_attn_dbg) { VS_CHECK_CUDA(cudaMalloc(&g_attn_dbg, 256 * 16 * sizeof(unsigned long long))); }
-      VS_CHECK_CUDA(cudaMemsetAsync(g_attn_dbg, 0, 256 * 16 * sizeof(unsigned long long), st));
-      a.dbg = g_attn_dbg;
-    }
-    return launch_pdl(attn_tcp_kernel<D, HO, NPOLY, EPIWG, DBG, PP, PTMEM>, dim3(ctas), dim3(EPIWG ? ATT_THREADS + 128 : ATT_THREADS), SMEM_P, st, 1, a);
-  }
-  else {
-    dim3 grid(a.n_qblk, heads, batch);
-    return launch_pdl(attn_tc_kernel<D, HO>, grid, dim3(ATT_THREADS), C::SMEM, st, 1, a);
-  }
+  dim3 grid((nq + TQ - 1) / TQ, heads, batch);
+  return launch_pdl(attn_tc_kernel<D>, grid, dim3(ATT_THREADS), C::SMEM, st, 1, a);
 }
 
 }  // namespace
 
-int attention_debug_read(unsigned long long* host, int n) {
-  if (!g_attn_dbg) return 1;
-  return cudaMemcpy(host, g_attn_dbg, (size_t)n * sizeof(unsigned long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
-}
-
-// Returns -1 when the shape is not handled by the tcgen05 kernel (caller falls back to the mma.sync kernel).
+// Returns -1 when the shape is not handled by the wgmma kernel (caller uses the mma.sync kernel).
 int attention_tc(cudaStream_t st, const __half* q, int ldq, const __half* k, int ldk, const __half* v, int ldv, __half* o,
                  int ldo, int batch, int nq, int nk, int heads, int d, long long q_bs, long long kv_bs, long long o_bs,
                  int kv_div) {
-  if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8)) return -1;
+  if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 2)) return -1;
   if ((q_bs % 8) || (kv_bs % 8)) return -1;
-#define VS_ATT_ARGS st, q, ldq, k, ldk, v, ldv, o, ldo, batch, nq, nk, heads, q_bs, kv_bs, o_bs, kv_div
-  // "attn_handoff" (A/B switch): 1 = the softmax ping-pong hands the MUFU pipe over after key chunk 6 of 8 (L0 self-
-  // attention 1549 us), 0 = after the last exponential (1607 us; interleaved repetitions on one box).
-  const bool early = get_option("attn_handoff") != 0;
-  // "attn_persist" (default 1): the persistent kernel with two issuer warps.  With the single issuer of round 1 it only won
-  // on short key sequences (profiles/r02_attn_ab_persistent_v1.json); with Q K^T and P V issued by two warps it wins
-  // everywhere (L0 self 1461 vs 1540 us, L1 self 138 vs 191 us, L0 cross 99 vs 183 us; profiles/r02_attn_ab_split_issuer.json).
-  // 0 = round-1 kernel (one CTA per work item, one issuer warp).
-  // Shipped configuration of the persistent kernel: P through tensor memory ("attn_ptmem" 1: L0 self 1422 vs 1458 us, L1
-  // self 134 vs 141 us, profiles/r02_attn_ab_ptmem.json), epilogue warpgroup for d = 40 ("attn_epiwg" 1), MUFU ping-pong
-  // ("attn_pingpong" 1), one FMA-pipe exp2 chunk of eight ("attn_poly" 1).  Any other setting of those switches selects
-  // the corresponding shared-memory-P A/B variant below.
-  if (get_option("attn_persist") != 0) {
-    const int np = get_option("attn_poly");
-    const bool epiwg = get_option("attn_epiwg") != 0, pingpong = get_option("attn_pingpong") != 0;
-    if (d == 40 && get_option("attn_debug") != 0)           // cycle counters (vs_debug_read)
-      return epiwg ? launch<40, 6, 0, true, true, true>(VS_ATT_ARGS) : launch<40, 6, 0, true, false, true>(VS_ATT_ARGS);
-    if (get_option("attn_ptmem") != 0 && pingpong && epiwg && np <= 1) {
-      if (d == 40) return np > 0 ? launch<40, 6, 1, true, true, false, true, true>(VS_ATT_ARGS) : launch<40, 6, 0, true, true, false, true, true>(VS_ATT_ARGS);
-      if (d == 80) return launch<80, 6, 0, true, false, false, true, true>(VS_ATT_ARGS);
-    }
-    if (!pingpong) {                               // A/B: softmax warpgroups free-running on the MUFU pipe
-      if (d == 40) return np > 0 ? launch<40, 6, 2, true, true, false, false>(VS_ATT_ARGS) : launch<40, 6, 0, true, true, false, false>(VS_ATT_ARGS);
-      if (d == 80) return launch<80, 6, 0, true, false, false, false>(VS_ATT_ARGS);
-    }
-    if (d == 40 && epiwg) {
-      switch (np) {
-        case 0: return launch<40, 6, 0, true, true>(VS_ATT_ARGS);
-        case 1: return launch<40, 6, 1, true, true>(VS_ATT_ARGS);
-        default: return launch<40, 6, 2, true, true>(VS_ATT_ARGS);
-      }
-    }
-    if (d == 40) {
-      switch (np) {
-        case 0: return launch<40, 6, 0, true>(VS_ATT_ARGS);
-        case 1: return launch<40, 6, 1, true>(VS_ATT_ARGS);
-        case 3: return launch<40, 6, 3, true>(VS_ATT_ARGS);
-        default: return launch<40, 6, 2, true>(VS_ATT_ARGS);
-      }
-    }
-    if (d == 80) return np > 1 ? launch<80, 6, 2, true>(VS_ATT_ARGS) : launch<80, 6, 0, true>(VS_ATT_ARGS);
-    return -1;
-  }
-  if (d == 40) return early ? launch<40, 6, 0, false>(VS_ATT_ARGS) : launch<40, 7, 0, false>(VS_ATT_ARGS);
-  if (d == 80) return early ? launch<80, 6, 0, false>(VS_ATT_ARGS) : launch<80, 7, 0, false>(VS_ATT_ARGS);
-#undef VS_ATT_ARGS
+  if (d == 40) return launch<40>(st, q, ldq, k, ldk, v, ldv, o, ldo, batch, nq, nk, heads, q_bs, kv_bs, o_bs, kv_div);
+  if (d == 80) return launch<80>(st, q, ldq, k, ldk, v, ldv, o, ldo, batch, nq, nk, heads, q_bs, kv_bs, o_bs, kv_div);
   return -1;
 }
 

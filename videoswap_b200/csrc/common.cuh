@@ -1,4 +1,4 @@
-// Shared device/host helpers for the sm_100a kernels: error handling, mbarrier / TMA / tcgen05 PTX wrappers.
+// Shared device/host helpers for the sm_90a kernels: error handling, mbarrier / TMA / wgmma PTX wrappers.
 // Hand-written inline PTX; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>          // CUtensorMap (types only; the driver entry point is fetched at run time)
@@ -141,7 +141,7 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// One lane of a fully converged warp.  The single-issuer roles (TMA producer, tcgen05.mma issuer) run their loops with
+// One lane of a fully converged warp.  The single-issuer roles (TMA producers) run their loops with
 // the WHOLE warp and predicate only the issuing instructions on this, so that addresses / descriptors stay warp-uniform
 // (uniform registers) instead of being re-broadcast through ELECT / VOTE / R2UR sequences inside a divergent branch.
 __device__ __forceinline__ bool elect_one() {
@@ -164,6 +164,12 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// shared::cluster address of `addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+  return r;
+}
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -172,122 +178,95 @@ __device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
 }
 
 // ---- programmatic dependent launch.  A kernel launched with launch_pdl() may start while its predecessor in the stream
-// is still draining: everything before pdl_wait() (barrier init, TMEM allocation, descriptor prefetch) overlaps the
+// is still draining: everything before pdl_wait() (barrier init, descriptor prefetch) overlaps the
 // predecessor's tail; pdl_wait() returns once the predecessor grid has completed and its memory is visible, so NO global
 // memory may be read or written before it.  pdl_trigger() lets the successor start being scheduled.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// ---- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 (fp16/bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- CTA pairs (cta_group::2): one tcgen05.mma of M = 256 spans the tensor cores, TMEM and shared memory of the two
-// CTAs of a cluster.  CTA r holds rows [128 r, 128 r + 128) of A and of the accumulator and rows [N/2 r, N/2 r + N/2)
-// of B; only the leader (rank 0) issues the MMA and its commits arrive on the barriers of both CTAs.
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t dst_smem, uint32_t ncols) {   // executed by the same warp of BOTH CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(mask) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// shared::cluster address of `addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {   // arrive on a (possibly remote) barrier
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads of a CTA pair: the data lands in THIS CTA's shared memory, the bytes are credited to `bar_cluster`
-// (a shared::cluster address, normally the leader's full barrier)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar_cluster, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const CUtensorMap* m, uint32_t bar_cluster, int c0, int c1,
-                                                 int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns: thread i of the warp receives lane (base+i), columns c..c+15.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// ---- warpgroup register reallocation: a producer warpgroup that only issues TMA hands registers to the MMA warpgroups
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
-// Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows are 128 B (64 fp16) apart inside an
-// 8-row swizzle atom, atoms are SBO = 1024 B apart.  (Bit layout: cute/arch/mma_sm100_desc.hpp SmemDescriptor.)
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
+// ---- wgmma (sm_90a warpgroup MMA): D[registers] (+)= A[smem desc] * B[smem desc], fp16 in, fp32 accumulate
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// Shared-memory matrix descriptor of a K-major operand with 128-byte swizzle: rows are 128 B (64 fp16) apart inside an
+// 8-row swizzle atom, atoms are SBO = 1024 B apart.  Advancing K by 16 elements adds 2 (32 bytes) to the address field.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address, 16-byte units
   d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                        // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                        // layout type: SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                        // layout type: SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16: fp16 x fp16 -> fp32, both operands K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4)                     // D format = F32
-         | (0u << 7) | (0u << 10)      // A, B format = F16
-         | (0u << 15) | (0u << 16)     // A, B K-major
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// MN-major operand with 128-byte swizzle (e.g. V [keys][64 channels] as the B operand of P V): 8-key groups are
+// SBO = 1024 B apart, 64-channel column blocks LBO apart.
+__device__ __forceinline__ uint64_t gmma_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
 }
+
+#define VS_R8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// m64n64k16: 32 fp32 accumulators per thread.  Register i holds row 16 w + lane / 4 + 8 ((i >> 1) & 1) of the warpgroup's
+// 64 rows (w = warp in the warpgroup) and column 8 (i >> 2) + 2 (lane & 3) + (i & 1).  tnspB = 1: B is MN-major.
+template <int TB = 0>
+__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "%32, %33, p, 1, 1, 0, %35;\n\t}"
+      : VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24)
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
+}
+template <int TB = 0>
+__device__ __forceinline__ void wgmma_m64n32(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, %19;\n\t}"
+      : VS_R8(0), VS_R8(8)
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
+}
+template <int TB = 0>
+__device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, %11;\n\t}"
+      : VS_R8(0)
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
+}
+// A from registers (four fp16x2 per thread in the m16n8k16 A-fragment layout of each warp's 16 rows), B from smem.
+template <int TB = 0>
+__device__ __forceinline__ void wgmma_m64n64_rs(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+      "{%32,%33,%34,%35}, %36, p, 1, 1, %38;\n\t}"
+      : VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
+}
+template <int TB = 0>
+__device__ __forceinline__ void wgmma_m64n16_rs(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, %14;\n\t}"
+      : VS_R8(0)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
+}
+#undef VS_R8
 
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.f + __expf(-x)); }   // 2 MUFU + 3 FP32
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }

@@ -1,26 +1,18 @@
-// tcgen05 / TMEM / TMA GEMM and implicit-GEMM 3x3 convolution for sm_100a.
+// wgmma / TMA GEMM and implicit-GEMM 3x3 convolution for sm_90a.
 //
-// One persistent, warp-specialised kernel:  warp 0 = TMA producer, warp 1 = tcgen05.mma issuer, warp 2 = TMEM allocator,
-// warps 4..11 = two epilogue warpgroups.  Tiles are 128 (M) x BN (N) x 64 (K, one 128-byte swizzle row of fp16);
-// accumulators are double-buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
+// One persistent, warp-specialised kernel of three warpgroups: warpgroup 0 is the TMA producer (one elected thread of
+// warp 0 issues the copies; the warpgroup gives most of its registers to the others with setmaxnreg), warpgroups 1 and 2
+// are the consumers: each owns 64 rows of the 128 (M) x BN (N) tile, issues wgmma.m64nNk16 on the 128-byte-swizzled
+// operand ring in shared memory and keeps its accumulator in registers.  K advances 64 elements (one swizzle row of
+// fp16) per ring stage; the producer runs up to STAGES k-blocks ahead, across tile boundaries, so the next tile's
+// operands are in flight while the consumers run the epilogue of the current one.
 // A 3x3 convolution is the same kernel with nine K segments: tap (dy,dx) loads the NHWC activation box shifted by
 // (dy,dx) through a 4-D TMA descriptor and the out-of-bounds zero fill of TMA provides the padding; a channel concat
 // is two descriptors walked back to back along K.
 //
-// What bounds it (ncu, see DESIGN.md section 7):
-//  * main loop: the L2 -> SM operand feed.  A 128 x 160 tile needs 36 KB per k-block (320 tensor cycles); every shape
-//    measured -- GEMM, conv, any K -- plateaus where that feed is ~45-60 B/clk/SM, i.e. ~55% of the tensor pipe.  Wider
-//    tiles need fewer bytes per flop, so BN is picked per shape by a wave-quantisation x bytes-per-k-block model
-//    (BN = 256: 48 KB per 512 tensor cycles) and, for K >= 768, two CTAs of a cluster share one 256-row tile with
-//    cta_group::2 MMAs (PAIR: each CTA loads half of the weight tile, 32 KB per 512 tensor cycles).
-//  * K <= 640: the epilogue.  With two epilogue warps per scheduler it is bound by the serial instruction stream of each
-//    warp, so the epilogue is specialised at compile time (GEGLU / residual / row vector), epilogue group g owns
-//    accumulator stage g (whole tiles: the per-tile set-up is paid once), and its body is kept small.
-//
-// Epilogue: TMEM -> registers (thread = output row) -> [folded LayerNorm: rstd * acc - rstd * mean * u] + bias (+ warp-
-// uniform time-embedding / positional row vector; both come from a per-warp shared-memory slice) / GEGLU -> fp16 -> warp-
-// private swizzled shared-memory transpose -> (+ fp16 residual, loaded coalesced one sub-tile ahead) -> coalesced 16-byte
-// global stores.  Tiny-N outputs (conv_out, N = 4) keep a direct-store path.
+// Epilogue (per consumer warp, 16 rows): registers -> [folded LayerNorm: rstd * acc - rstd * mean * u] + bias (+ time-
+// embedding / positional row vector) / GEGLU -> fp16 -> warp-private swizzled shared-memory transpose, 32 columns at a
+// time -> (+ fp16 residual) -> coalesced 16-byte global stores.  Tiny-N outputs (conv_out, N = 4) keep a direct-store path.
 //
 // Replaces (reference call sites): InflatedConv3d 3x3 / 1x1 (models/animatediff_models/resnet.py:9-18), every
 // nn.Linear / 1x1 conv of Transformer3DModel (attention.py:65-93,174-204) and the motion module
@@ -35,12 +27,13 @@ namespace {
 constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
-constexpr int GEMM_THREADS = 384;                   // 4 control warps + 2 epilogue warpgroups
+constexpr int GEMM_THREADS = 384;                   // producer warpgroup + 2 consumer warpgroups
 constexpr int SMEM_LIMIT = 227 * 1024;
-constexpr int EPI_COLS = 32;                        // output columns per epilogue sub-tile (64 B of fp16: SWIZZLE_64B)
-constexpr int EPI_WARP_BYTES = 4096;                // per epilogue warp: 2 KB transpose staging + 1 KB bias + 1 KB LN-fold slice
+constexpr int EPI_COLS = 32;                        // output columns per epilogue sub-tile (64 B of fp16)
+constexpr int EPI_WARP_BYTES = 16 * 64;             // per consumer warp: [16 rows x 64 B] transpose staging
 constexpr int EPI_BYTES = 8 * EPI_WARP_BYTES;
-enum { EPI_F_GEGLU = 1, EPI_F_RES = 2, EPI_F_RV = 4, EPI_F_LN = 8, EPI_F_LNOUT = 16, EPI_F_RESST = 32 };   // compile-time epilogue features
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
+enum { EPI_F_GEGLU = 1, EPI_F_RES = 2, EPI_F_RV = 4, EPI_F_LN = 8, EPI_F_LNOUT = 16 };   // compile-time epilogue features
 
 struct GemmParams {
   CUtensorMap tmA, tmA2, tmB;
@@ -70,140 +63,94 @@ struct GemmParams {
   int ldr;
   __half* out;
   int ldc;
-  int epi_prefetch;  // 1 = the accumulator columns of sub-tile s+1 are loaded from TMEM while sub-tile s is processed
-  int res_stage;     // 1 = linear layers with a residual and K <= 320 keep the residual tile in shared memory (EPI_F_RESST)
-  int res_prefetch;  // residual rows of this epilogue group's NEXT tile are prefetched into L2 while the current tile is
-                     // drained: 1 = prefetch.global.L2 per 128 bytes, 2 = one cp.async.bulk.prefetch.L2 per row, 0 = off
   int staged;        // 1 = smem-transposed coalesced epilogue; 0 = direct stores for tiny / unaligned N
   int stages;        // 0 = all, else limits the smem ring depth (pipeline-depth experiments)
 };
 
-// RESST: the epilogue keeps the residual rows of a whole tile in shared memory (one private [32 rows x BN] slice per epilogue
-// warp, filled with cp.async a whole tile ahead); it costs ring stages, so only tiles up to BN = 160 take it.
-template <int BN, bool PAIR = false, bool RESST = false>
+template <int BN>
 struct Cfg {
-  static constexpr int B_STAGE_BYTES = (PAIR ? BN / 2 : BN) * BK * 2;   // a CTA pair splits the weight tile along N
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  // row stride of a residual slice: 64 B of padding when the row would be a multiple of 128 B, so that the two rows a
-  // quarter-warp reads per LDS.128 phase fall into different bank halves
-  static constexpr int RES_ROW_BYTES = BN * 2 + ((BN * 2) % 128 == 0 ? 64 : 0);
-  static constexpr int RES_WARP_BYTES = RESST ? 32 * RES_ROW_BYTES : 0;
-  static constexpr int RES_BYTES = 8 * RES_WARP_BYTES;
-  static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES - RES_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + RES_BYTES;
-  static_assert(2 * BN <= 512, "two accumulator stages must fit TMEM");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(B_STAGE_BYTES % 1024 == 0, "B stage must keep 1024-byte alignment for SWIZZLE_128B");
   static_assert(STAGES >= 3, "pipeline too shallow");
+  static_assert(BN % 32 == 0 && BN <= 256, "wgmma N");
 };
 
-__host__ __device__ constexpr bool residual_staged(int BN, int EPI) {
-  return (EPI & EPI_F_RESST) != 0 && (EPI & EPI_F_RES) != 0 && (EPI & EPI_F_GEGLU) == 0 && BN <= 160;
-}
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ uint32_t sw64_off(int row, int chunk) {   // byte offset inside a [32 x 64 B] SWIZZLE_64B tile
+__device__ __forceinline__ uint32_t sw64_off(int row, int chunk) {   // byte offset inside a [rows x 64 B] swizzled tile
   return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4));
 }
 
-// PAIR: two CTAs of a cluster (an SM pair) compute a 256 x BN tile with cta_group::2 MMAs: each loads its own 128 rows
-// of A and HALF of the weight tile, so the L2 -> SM operand feed per flop -- the bound of the main loop -- drops by a
-// third (BN = 256: 32 KB instead of 48 KB per 512 tensor cycles and CTA).
-template <int BN, int EPI, bool PAIR>
+// acc (+)= A[64 rows] B[BN rows]^T over one k16 step: BN / 64 m64n64 instructions and one m64n32 for the rest.
+template <int BN>
+__device__ __forceinline__ void mma_k16(float* acc, uint64_t da, uint64_t db, uint32_t scale_d) {
+#pragma unroll
+  for (int c = 0; c < BN / 64; ++c) wgmma_m64n64(acc + 32 * c, da, db + (uint64_t)(c * 64 * 128 / 16), scale_d);
+  if (BN % 64) wgmma_m64n32(acc + 32 * (BN / 64), da, db + (uint64_t)((BN / 64) * 64 * 128 / 16), scale_d);
+}
+
+template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
-  constexpr bool RESST = residual_staged(BN, EPI);
-  using C = Cfg<BN, PAIR, RESST>;
+  using C = Cfg<BN>;
   constexpr bool GEGLU = (EPI & EPI_F_GEGLU) != 0, HAS_RES = (EPI & EPI_F_RES) != 0, HAS_RV = (EPI & EPI_F_RV) != 0;
   // LN: the A operand is the RAW input of a LayerNorm whose affine map is folded into the weights:
   //   LN(x) W^T = rstd (x W'^T) - rstd mean u + c,  W' = W * gamma, u[n] = sum_k W'[n,k], c = beta W^T + bias (the `bias`)
   constexpr bool LN = (EPI & EPI_F_LN) != 0;
   // LNOUT: this GEMM's output feeds a LayerNorm (folded into the NEXT GEMM): the row statistics of what is stored -- the
   // fp16-rounded values, after the residual add -- are accumulated here, in the shadow of the store path, and written as
-  // one (sum, sum of squares) pair per (column tile, row).  Deterministic (no atomics); replaces the stand-alone
-  // ln_stats_kernel pass, which re-read every such tensor from HBM (4.5 GB per step).
+  // one (sum, sum of squares) pair per (column tile, row).  Deterministic (no atomics); replaces a stand-alone statistics
+  // pass that would re-read every such tensor from HBM.
   constexpr bool LNOUT = (EPI & EPI_F_LNOUT) != 0;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t epi_base = smem_base + C::STAGES * C::STAGE_BYTES;
   const uint32_t bar_base = epi_base + EPI_BYTES;
-  // barrier layout: full[S], empty[S], tmem_full[2], tmem_empty[2], then the TMEM base address word
+  // barrier layout: full[S], empty[S]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint32_t* tmem_slot_ptr = reinterpret_cast<uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t crank = PAIR ? cluster_ctarank() : 0u;        // 0 = leader (issues the MMAs)
-  const int total_tiles = (PAIR ? (p.m_tiles + 1) / 2 : p.m_tiles) * p.n_tiles;   // PAIR: tiles of 256 rows
+  const int wg = threadIdx.x >> 7;
+  const int total_tiles = p.m_tiles * p.n_tiles;
   const int nst = (p.stages > 0 && p.stages < C::STAGES) ? p.stages : C::STAGES;   // ring depth (debug knob: "gemm_stages")
   // Tile order: n fastest, tiles round-robin over the CTAs (CTAs running at the same time share the A row panel and a
-  // few weight tiles in L2).  m-fastest and operand-stationary orders measured 3-40% slower.
-  const int t_begin = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, t_step = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
+  // few weight tiles in L2).
+  const int t_begin = blockIdx.x, t_step = gridDim.x;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&p.tmA);
     prefetch_tmap(&p.tmB);
     if (p.kb_src1 < p.kb_per_tap) prefetch_tmap(&p.tmA2);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), PAIR ? 256 : 128);   // one epilogue warpgroup per accumulator stage (of each CTA)
+      mbar_init(empty_bar(s), 8);                // one arrival per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if (PAIR) tmem_alloc_pair(tmem_slot, C::TMEM_COLS);
-    else tmem_alloc(tmem_slot, C::TMEM_COLS);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();                  // the peer's barriers are initialised before any remote arrive / TMA credit
-  tc_fence_after();
   pdl_trigger();                                 // the next kernel may start its own set-up
   pdl_wait();                                    // everything above overlapped the previous kernel's tail; its data is visible now
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
-  // The two single-issuer roles below run with the WHOLE warp (all values warp-uniform) and predicate only the issuing
-  // instructions on one elected lane.  ncu showed that with the loops inside `if (lane == 0)` the MMA warp spent ~95% of
-  // the kernel executing its own 129-instruction loop body (ELECT / VOTEU / R2UR.BROADCAST sequences re-materialising
-  // the descriptors in uniform registers) and capped the tensor pipe at 44%; the loops also carry no division / modulo.
-  if (warp == 0) {
-    // =================================================================== TMA producer
+  if (wg == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp != 0) return;
+    // =================================================================== TMA producer (whole warp, one elected issuer)
     const int num_kb = p.num_kb, kb_per_tap = p.kb_per_tap, kb_src1 = p.kb_src1;
     const bool conv = p.a_rank == 4;
     const int tap_x0 = p.tap_x0, tap_x1 = p.tap_x0 + p.tap_w;
     uint32_t pr_s = 0, pr_ph = 0;              // ring stage / phase, carried across tiles
     for (int tile = t_begin; tile < total_tiles; tile += t_step) {
-      const int mt = tile / p.n_tiles, n_tile = tile - mt * p.n_tiles;
-      const int m_tile = PAIR ? 2 * mt + (int)crank : mt;      // may be == m_tiles (odd count): an all-out-of-bounds tile
+      const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
       int x0 = 0, y0 = 0, i0 = 0;
       if (conv) {
         x0 = (m_tile % p.tiles_x) * p.TW;
         y0 = ((m_tile / p.tiles_x) % p.tiles_y) * p.TH;
         i0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.TN;
       }
-      const int n0 = n_tile * BN + (PAIR ? (int)crank * (BN / 2) : 0);   // PAIR: this CTA's half of the weight tile
+      const int n0 = n_tile * BN;
       const int m0 = m_tile * BM;
       int kcoord = 0;                          // K coordinate into the weight panel (kb * 64)
       int dy = p.tap_y0, dx = tap_x0;          // tap offsets, advanced like an odometer
@@ -216,18 +163,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
           const bool first = r < kb_src1;
           const CUtensorMap* tm = first ? &p.tmA : &p.tmA2;
           const int c = (first ? r : r - kb_src1) * BK;
-          if (PAIR) {                          // both CTAs' bytes are credited to the LEADER's full barrier
-            const uint32_t fbl = mapa_shared(fb, 0);
-            if (crank == 0) mbar_expect_tx(fb, 2 * C::STAGE_BYTES);
-            if (conv) tma_load_4d_pair(a_dst, tm, fbl, c, x0 + dx, y0 + dy, i0);
-            else tma_load_2d_pair(a_dst, tm, fbl, c, m0);
-            tma_load_2d_pair(a_dst + A_STAGE_BYTES, &p.tmB, fbl, kcoord, n0);
-          } else {
-            mbar_expect_tx(fb, C::STAGE_BYTES);
-            if (conv) tma_load_4d(a_dst, tm, fb, c, x0 + dx, y0 + dy, i0);
-            else tma_load_2d(a_dst, tm, fb, c, m0);
-            tma_load_2d(a_dst + A_STAGE_BYTES, &p.tmB, fb, kcoord, n0);
-          }
+          mbar_expect_tx(fb, C::STAGE_BYTES);
+          if (conv) tma_load_4d(a_dst, tm, fb, c, x0 + dx, y0 + dy, i0);
+          else tma_load_2d(a_dst, tm, fb, c, m0);
+          tma_load_2d(a_dst + A_STAGE_BYTES, &p.tmB, fb, kcoord, n0);
         }
         __syncwarp();
         kcoord += BK;
@@ -238,414 +177,206 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         if (++pr_s == (uint32_t)nst) { pr_s = 0; pr_ph ^= 1; }
       }
     }
-  } else if (warp == 1 && crank == 0) {
-    // =================================================================== MMA issuer (PAIR: the leader CTA only)
-    constexpr uint32_t idesc = umma_idesc_f16(PAIR ? 2 * BM : BM, BN);
-    const int num_kb = p.num_kb;
-    uint32_t mm_s = 0, mm_ph = 0, t = 0;
-    for (int tile = t_begin; tile < total_tiles; tile += t_step, ++t) {
-      const int acc = t & 1;
-      const uint32_t aph = (t >> 1) & 1;
-      mbar_wait(tempty_bar(acc), aph ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(full_bar(mm_s), mm_ph);
-        tc_fence_after();
-        if (elect_one()) {
-          // one descriptor per operand per k-block; the K = 16 sub-steps advance the 16-byte-unit address field by 2
-          const uint32_t a_addr = smem_base + mm_s * C::STAGE_BYTES;
-          const uint64_t ad = umma_desc_sw128_kmajor(a_addr);
-          const uint64_t bd = umma_desc_sw128_kmajor(a_addr + A_STAGE_BYTES);
-          if (PAIR) {
-            tc_mma_f16_pair(d_tmem, ad, bd, idesc, kb != 0 ? 1u : 0u);
-            tc_mma_f16_pair(d_tmem, ad + 2, bd + 2, idesc, 1u);
-            tc_mma_f16_pair(d_tmem, ad + 4, bd + 4, idesc, 1u);
-            tc_mma_f16_pair(d_tmem, ad + 6, bd + 6, idesc, 1u);
-            tc_commit_pair(empty_bar(mm_s), (uint16_t)0x3);   // frees the slot in BOTH CTAs
-            if (kb == num_kb - 1) tc_commit_pair(tfull_bar(acc), (uint16_t)0x3);
-          } else {
-            tc_mma_f16(d_tmem, ad, bd, idesc, kb != 0 ? 1u : 0u);
-            tc_mma_f16(d_tmem, ad + 2, bd + 2, idesc, 1u);
-            tc_mma_f16(d_tmem, ad + 4, bd + 4, idesc, 1u);
-            tc_mma_f16(d_tmem, ad + 6, bd + 6, idesc, 1u);
-            tc_commit(empty_bar(mm_s));        // frees the smem slot once these MMAs have read it
-            if (kb == num_kb - 1) tc_commit(tfull_bar(acc));   // accumulator complete -> epilogue
-          }
-        }
-        __syncwarp();
-        if (++mm_s == (uint32_t)nst) { mm_s = 0; mm_ph ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // =================================================================== epilogue
-    // Warpgroup g drains accumulator stage g, i.e. every second tile of this CTA.
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int row = q * 32 + lane;          // row of the tile handled by this thread
-    const int grp = (warp - 4) >> 2;
-    const int acc = grp;
-    const uint32_t out_stage = epi_base + (warp - 4) * EPI_WARP_BYTES, bias_stage = out_stage + 2048, u_stage = bias_stage + 1024;
-    const int tr = lane >> 2, tch = lane & 3;   // transposed mapping: 8 rows x four 16-byte chunks per instruction
-    const bool has_bias = p.bias != nullptr;
-    const bool staged = p.staged != 0;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN;
-    uint32_t aph = 0;
-    const uint32_t tempty_arrive = PAIR ? mapa_shared(tempty_bar(acc), 0) : tempty_bar(acc);   // PAIR: the leader's barrier
-    // output pixel (row of the GEMM) this thread owns in `tile`, -1 = outside the problem
-    auto tile_pixel = [&](int tile, int& n_tile) -> int {
-      const int mt = tile / p.n_tiles;
-      n_tile = tile - mt * p.n_tiles;
-      const int m_tile = PAIR ? 2 * mt + (int)crank : mt;
-      if (p.a_rank == 4) {
-        const int x0 = (m_tile % p.tiles_x) * p.TW;
-        const int y0 = ((m_tile / p.tiles_x) % p.tiles_y) * p.TH;
-        const int i0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.TN;
-        const int ti = row >> p.thw_log, rem = row & ((1 << p.thw_log) - 1);
-        const int y = y0 + (rem >> p.tw_log), x = x0 + (rem & (p.TW - 1)), img = i0 + ti;
-        return ((m_tile < p.m_tiles) && (img < p.nimg) && (y < p.H) && (x < p.W))
-                   ? (img * p.OH + y * p.osy + p.ooy) * p.OW + x * p.osx + p.oox : -1;
-      }
-      const int px = m_tile * BM + row;
-      return px < p.M ? px : -1;
-    };
-    // The residual add made the K <= 640 epilogues DRAM-latency-bound: each 32-column sub-tile waited for residual rows
-    // requested only one sub-tile earlier (ncu: the top stall of the epilogue warps was the long scoreboard on those loads,
-    // DRAM at 46 %, tensor pipe at 22 %).  The rows of the group's NEXT tile are therefore pulled into L2 a whole tile ahead.
-    auto prefetch_residual = [&](int tile) {
-      if (tile >= total_tiles) return;
-      int nt;
-      const int px = tile_pixel(tile, nt);
-      if (px < 0) return;
-      const int n0p = nt * BN;
-      const int bytes = (p.N - n0p < BN ? p.N - n0p : BN) * 2;
-      const char* src = reinterpret_cast<const char*>(p.residual + (long long)px * p.ldr + n0p);
-      if (p.res_prefetch == 2) {
-        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-      } else {
-        for (int o = 0; o < bytes; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(src + o));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(src + bytes - 1));
-      }
-    };
-    const bool res_pf = HAS_RES && !GEGLU && !RESST && staged && p.res_prefetch != 0;
-    if (res_pf) prefetch_residual(t_begin + grp * t_step);
-    // RESST -- whole-tile residual stage.  With the residual rows requested one 32-column sub-tile ahead (register double
-    // buffer, below) every epilogue warp sat out one full memory latency per sub-tile: 5 x ~1.2 us + work = the 8.6 us a
-    // BN = 160 tile took (64 us vs 42 us without the residual at M = 131072, N = K = 320; fewer instructions or an L2
-    // prefetch did not move it; this stage brings it to 58 us -- it costs ring stages, see launch_linear for where it is used).  Now each lane owns the sixteen-byte
-    // chunks it will add after the transpose -- rows i*8 + tr, chunk tch of every sub-tile -- in a private shared-memory
-    // slice: it copies them in with cp.async, one commit group per sub-tile, and refills a sub-tile's chunks with the NEXT
-    // tile's rows right after it has consumed them.  A chunk is written and read by the same lane only, so no barrier is
-    // involved: program order covers write-after-read, cp.async.wait_group covers read-after-write.  Every tile commits
-    // exactly MAXSUB groups (empty ones for missing sub-tiles or a missing next tile), so when sub-tile s is consumed the
-    // groups younger than its own are always MAXSUB - 1: (MAXSUB - 1 - s) of this tile + s refills.
-    constexpr int MAXSUB_T = (GEGLU ? BN / 2 : BN) / EPI_COLS;
-    const uint32_t res_lane = bar_base + 256u + (uint32_t)((warp - 4) * C::RES_WARP_BYTES + tr * C::RES_ROW_BYTES + tch * 16);
-    const __half* rnext[4] = {nullptr, nullptr, nullptr, nullptr};   // this lane's 4 residual rows of the group's next tile
-    int nsub_next = 0;
-    auto residual_rows = [&](int tile) {
-      nsub_next = 0;
-      if (tile < total_tiles) {               // warp-uniform
-        int nt;
-        const int px = tile_pixel(tile, nt);
-        const int n0p = nt * BN;
-        nsub_next = (p.N - n0p < BN ? p.N - n0p : BN) / EPI_COLS;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int tp = __shfl_sync(0xffffffffu, px, i * 8 + tr);
-          rnext[i] = tp >= 0 ? p.residual + (long long)tp * p.ldr + n0p + tch * 8 : nullptr;
-        }
-      }
-    };
-    auto stage_residual = [&](int s) {       // this lane's chunks of sub-tile s of the next tile; always exactly one group
-      if (s < nsub_next) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          if (rnext[i] != nullptr) cp_async16(res_lane + (uint32_t)(i * 8 * C::RES_ROW_BYTES + s * 64), rnext[i] + s * EPI_COLS);
-      }
-      cp_async_commit();
-    };
-    if (RESST && staged) {
-      residual_rows(t_begin + grp * t_step);
-#pragma unroll 1
-      for (int s = 0; s < MAXSUB_T; ++s) stage_residual(s);
-    }
-    for (int tile = t_begin + grp * t_step; tile < total_tiles; tile += 2 * t_step, aph ^= 1) {
-      int n_tile;
-      const int pix = tile_pixel(tile, n_tile);
-      if (res_pf) prefetch_residual(tile + 2 * t_step);
-      if (RESST && staged) residual_rows(tile + 2 * t_step);
-      const int n0 = n_tile * BN;
+    return;
+  }
 
-      if (staged) {
-        constexpr int OC = GEGLU ? BN / 2 : BN;                            // output columns of a full tile
-        const int oc0 = n_tile * OC;                                        // first output column of this tile
-        const int nsub = (p.N - n0 < BN ? (GEGLU ? (p.N - n0) / 2 : p.N - n0) : OC) / EPI_COLS;
-        const float* rv = nullptr;
-        // Row vectors (time embedding per batch element, positional offsets per frame): the 32 rows of a warp nearly always
-        // share one vector, which is then folded into the warp's bias slice; mixed warps read theirs per sub-tile.
-        bool rv_uniform = false;
-        const float* rv_warp = nullptr;
-        if (HAS_RV) {
-          int ri = -1;
-          if (pix >= 0) {
-            ri = pix / p.pix_per_batch;
-            if (p.rv_mod > 0) ri %= p.rv_mod;
-            rv = p.rowvec + (long long)ri * p.ldrv + n0;
-          }
-          const unsigned live = __ballot_sync(0xffffffffu, pix >= 0);
-          if (live != 0u) {
-            const int r0 = __shfl_sync(0xffffffffu, ri, __ffs(live) - 1);
-            rv_uniform = __all_sync(0xffffffffu, pix < 0 || ri == r0);
-            rv_warp = p.rowvec + (long long)r0 * p.ldrv;
-          }
+  // ===================================================================== consumers: MMA + epilogue
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int g = wg - 1;                        // rows [64 g, 64 g + 64) of the tile
+  const int wq = warp & 3;                     // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of those
+  const int q = lane & 3;
+  const int rbase = 64 * g + 16 * wq + (lane >> 2);   // this thread's tile rows: rbase and rbase + 8
+  const uint32_t stage_buf = epi_base + (uint32_t)(warp - 4) * EPI_WARP_BYTES;
+  const bool has_bias = p.bias != nullptr;
+  const bool staged = p.staged != 0;
+  const int num_kb = p.num_kb;
+  // output pixel (row of the GEMM) of tile row `row`, -1 = outside the problem
+  auto tile_pixel = [&](int m_tile, int row) -> int {
+    if (p.a_rank == 4) {
+      const int x0 = (m_tile % p.tiles_x) * p.TW;
+      const int y0 = ((m_tile / p.tiles_x) % p.tiles_y) * p.TH;
+      const int i0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.TN;
+      const int ti = row >> p.thw_log, rem = row & ((1 << p.thw_log) - 1);
+      const int y = y0 + (rem >> p.tw_log), x = x0 + (rem & (p.TW - 1)), img = i0 + ti;
+      return ((img < p.nimg) && (y < p.H) && (x < p.W)) ? (img * p.OH + y * p.osy + p.ooy) * p.OW + x * p.osx + p.oox : -1;
+    }
+    const int px = m_tile * BM + row;
+    return px < p.M ? px : -1;
+  };
+
+  float acc[BN / 2];
+  uint32_t s = 0, ph = 0;
+  for (int tile = t_begin; tile < total_tiles; tile += t_step) {
+    // ------------------------------------------------------------------ main loop
+    uint32_t prev = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(full_bar(s), ph);
+      wgmma_fence();
+      const uint32_t a_addr = smem_base + s * C::STAGE_BYTES;
+      const uint64_t da = gmma_desc_sw128(a_addr + g * 64 * 128);
+      const uint64_t db = gmma_desc_sw128(a_addr + A_STAGE_BYTES);
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) mma_k16<BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      wgmma_commit();
+      if (kb > 0) {                            // the MMAs of the previous k-block have read their stage: release it
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(empty_bar(prev));
+      }
+      prev = s;
+      if (++s == (uint32_t)nst) { s = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(empty_bar(prev));
+
+    // ------------------------------------------------------------------ epilogue
+    const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
+    const int n0 = n_tile * BN;
+    int pix[2];
+    pix[0] = tile_pixel(m_tile, rbase);
+    pix[1] = tile_pixel(m_tile, rbase + 8);
+    const float* rv[2] = {nullptr, nullptr};
+    if (HAS_RV || !staged) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (p.rowvec != nullptr && pix[h] >= 0) {
+          int ri = pix[h] / p.pix_per_batch;
+          if (p.rv_mod > 0) ri %= p.rv_mod;
+          rv[h] = p.rowvec + (long long)ri * p.ldrv + n0;
         }
-        float la = 1.f, lb = 0.f;           // folded LayerNorm: row scale and row shift factor
-        if (LN && pix >= 0) {
+      }
+    }
+    if (staged) {
+      constexpr int OC = GEGLU ? BN / 2 : BN;                            // output columns of a full tile
+      const int oc0 = n_tile * OC;                                        // first output column of this tile
+      const int nsub = (p.N - n0 < BN ? (GEGLU ? (p.N - n0) / 2 : p.N - n0) : OC) / EPI_COLS;
+      float la[2] = {1.f, 1.f}, lb[2] = {0.f, 0.f};                      // folded LayerNorm: row scale and shift factor
+      if (LN) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (pix[h] < 0) continue;
           if (p.ln_nparts > 0) {            // statistics from the producer GEMM's per-column-tile partial sums
             float S = 0.f, Q = 0.f;
             for (int k = 0; k < p.ln_nparts; ++k) {
-              const float2 v = __ldg(p.ln_parts + (long long)k * p.M + pix);
+              const float2 v = __ldg(p.ln_parts + (long long)k * p.M + pix[h]);
               S += v.x; Q += v.y;
             }
             const float mean = S * p.ln_inv_c;
-            la = rsqrtf(fmaxf(fmaf(-mean, mean, Q * p.ln_inv_c), 0.f) + 1e-5f);
-            lb = -mean * la;
+            la[h] = rsqrtf(fmaxf(fmaf(-mean, mean, Q * p.ln_inv_c), 0.f) + 1e-5f);
+            lb[h] = -mean * la[h];
           } else {
-            const float2 st2 = __ldg(p.ln_stats + pix);
-            la = st2.x; lb = st2.y;
+            const float2 st2 = __ldg(p.ln_stats + pix[h]);
+            la[h] = st2.x; lb[h] = st2.y;
           }
         }
-        float rs[4] = {0.f, 0.f, 0.f, 0.f}, rq[4] = {0.f, 0.f, 0.f, 0.f};   // LNOUT: sums of the 4 rows this lane stores
-        int tpix[4];                        // pixels of the rows this lane stores after the transpose
+      }
+      float rs[2] = {0.f, 0.f}, rq[2] = {0.f, 0.f};   // LNOUT: sums of the 2 rows this lane stores
+      // After the transpose this lane stores 16-byte chunk q of its own two rows (rbase, rbase + 8).
+      __half* orow[2];
+      const __half* rrow[2];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) tpix[i] = __shfl_sync(0xffffffffu, pix, i * 8 + tr);
-        // Row pointers of the 4 rows this lane stores, computed once per tile: the sub-tile loop below is fully unrolled for
-        // the linear epilogues, so every access becomes [pointer + immediate].  (Computed per access inside a rolled loop --
-        // 64-bit multiplies, constant-bank reloads after every asm volatile, one branch per row, register copies for the
-        // residual double buffer -- the sub-tile body was ~300 instructions per warp; the diet to ~210 bought 2 % of the GEMM
-        // time, the residual latency above was the larger term: profiles/r02_ncu_proj.json, r02_epilogue_shapes_ab.json.)
-        // Rows outside the problem point at row 0 (loads are harmless, stores are predicated).
-        __half* orow[4];
-        const __half* rrow[4];
+      for (int h = 0; h < 2; ++h) {
+        const long long px = pix[h] >= 0 ? pix[h] : 0;     // rows outside the problem: loads harmless, stores predicated
+        orow[h] = p.out + px * p.ldc + oc0 + q * 8;
+        rrow[h] = HAS_RES ? p.residual + px * p.ldr + oc0 + q * 8 : nullptr;
+      }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const long long px = tpix[i] >= 0 ? tpix[i] : 0;
-          orow[i] = p.out + px * p.ldc + oc0 + tch * 8;
-          rrow[i] = (HAS_RES && !RESST) ? p.residual + px * p.ldr + oc0 + tch * 8 : nullptr;
+      for (int sb = 0; sb < OC / EPI_COLS; ++sb) {
+        if (sb >= nsub) break;                  // warp-uniform
+        uint4 rr[2];
+        if (HAS_RES) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) rr[h] = __ldg(reinterpret_cast<const uint4*>(rrow[h] + sb * EPI_COLS));
         }
-        // Residual rows are requested one sub-tile ahead of their use into the OTHER of two register sets (the sub-tile loop is
-        // unrolled by two so the sets alternate without copies).
-        uint4 res_a[4], res_b[4];
-        auto load_res = [&](int s, uint4 (&dst)[4]) {
 #pragma unroll
-          for (int i = 0; i < 4; ++i) dst[i] = __ldg(reinterpret_cast<const uint4*>(rrow[i] + s * EPI_COLS));
-        };
-        if (HAS_RES && !RESST) load_res(0, res_a);
-        // The tile's bias vector goes to this warp's own shared-memory slice while the accumulator is still being
-        // computed; the sub-tiles then read it as broadcast LDS.  (Read with __ldg inside the sub-tile loop, the epilogue
-        // warps of the K = 320 GEMMs spent 31% of their time waiting for those loads.)
-        const bool stage_bias = has_bias || (HAS_RV && rv_uniform);
-        if (stage_bias) {
-          __syncwarp();                     // the previous tile's readers are done
-#pragma unroll
-          for (int c = lane; c < BN / 4; c += 32) {
-            const int n = n0 + 4 * c;
-            float4 b = (has_bias && n + 3 < p.N) ? __ldg(reinterpret_cast<const float4*>(p.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            if (HAS_RV && rv_uniform && n + 3 < p.N) {
-              const float4 r4 = __ldg(reinterpret_cast<const float4*>(rv_warp + n));
-              b.x += r4.x; b.y += r4.y; b.z += r4.z; b.w += r4.w;
-            }
-            asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(bias_stage + 16 * c), "f"(b.x), "f"(b.y), "f"(b.z), "f"(b.w) : "memory");
-            if (LN) {
-              const float4 u4 = n + 3 < p.N ? __ldg(reinterpret_cast<const float4*>(p.ln_u + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(u_stage + 16 * c), "f"(u4.x), "f"(u4.y), "f"(u4.z), "f"(u4.w) : "memory");
-            }
+        for (int jj = 0; jj < 4; ++jj) {
+          const int j = 4 * sb + jj;            // n8 block of the (output) tile
+          const int c = 8 * j + 2 * q;          // column inside the tile (value column for GEGLU)
+          float2 b = has_bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
+          float2 u = LN ? __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + c)) : make_float2(0.f, 0.f);
+          float2 bg = make_float2(0.f, 0.f), ug = make_float2(0.f, 0.f);
+          if (GEGLU) {                          // gate columns are BN / 2 further on, in the same thread's registers
+            bg = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + BN / 2 + c));
+            if (LN) ug = __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + BN / 2 + c));
           }
-          __syncwarp();
-        }
-        mbar_wait(tfull_bar(acc), aph);
-        tc_fence_after();
-        // Linear epilogues prefetch the next 32 accumulator columns (tcgen05.ld is asynchronous until tcgen05.wait::ld), so the
-        // TMEM round trip of sub-tile s+1 overlaps the bias / transpose / store work of sub-tile s.
-        uint32_t vn[32];
-        const bool prefetch = !GEGLU && p.epi_prefetch != 0;
-        if (prefetch) tmem_ld32(taddr, vn);
-        auto subtile = [&](const int s, uint4 (&rcur)[4], uint4 (&rnxt)[4]) {
-          float f[32];
-          if (prefetch) {
-            tmem_ld_wait();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(vn[j]);
-            if (s + 1 < nsub) tmem_ld32(taddr + (s + 1) * EPI_COLS, vn);
-          } else {
-            uint32_t v[32];
-            tmem_ld32(taddr + s * EPI_COLS, v);
+          for (int h = 0; h < 2; ++h) {
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
             if (GEGLU) {
-              uint32_t g[32];
-              tmem_ld32(taddr + BN / 2 + s * EPI_COLS, g);
-              tmem_ld_wait();
-              const uint32_t bv = bias_stage + s * EPI_COLS * 4, bg = bv + (BN / 2) * 4;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 b = lds_f4(bv + j * 4);
-                float4 c = lds_f4(bg + j * 4);
-                if (LN) {                        // value / gate pre-activations of the folded LayerNorm
-                  const float4 uv = lds_f4(bv + 1024 + j * 4), ug = lds_f4(bg + 1024 + j * 4);
-                  b.x = fmaf(lb, uv.x, b.x); b.y = fmaf(lb, uv.y, b.y); b.z = fmaf(lb, uv.z, b.z); b.w = fmaf(lb, uv.w, b.w);
-                  c.x = fmaf(lb, ug.x, c.x); c.y = fmaf(lb, ug.y, c.y); c.z = fmaf(lb, ug.z, c.z); c.w = fmaf(lb, ug.w, c.w);
-#pragma unroll
-                  for (int t = 0; t < 4; ++t) {
-                    v[j + t] = __float_as_uint(__uint_as_float(v[j + t]) * la);
-                    g[j + t] = __float_as_uint(__uint_as_float(g[j + t]) * la);
-                  }
-                }
-                f[j] = (__uint_as_float(v[j]) + b.x) * gelu_sig(__uint_as_float(g[j]) + c.x);
-                f[j + 1] = (__uint_as_float(v[j + 1]) + b.y) * gelu_sig(__uint_as_float(g[j + 1]) + c.y);
-                f[j + 2] = (__uint_as_float(v[j + 2]) + b.z) * gelu_sig(__uint_as_float(g[j + 2]) + c.z);
-                f[j + 3] = (__uint_as_float(v[j + 3]) + b.w) * gelu_sig(__uint_as_float(g[j + 3]) + c.w);
+              float g0 = acc[4 * (j + BN / 16) + 2 * h], g1 = acc[4 * (j + BN / 16) + 2 * h + 1];
+              float bv0 = b.x, bv1 = b.y, bg0 = bg.x, bg1 = bg.y;
+              if (LN) {                         // value / gate pre-activations of the folded LayerNorm
+                bv0 = fmaf(lb[h], u.x, bv0); bv1 = fmaf(lb[h], u.y, bv1);
+                bg0 = fmaf(lb[h], ug.x, bg0); bg1 = fmaf(lb[h], ug.y, bg1);
+                f0 *= la[h]; f1 *= la[h]; g0 *= la[h]; g1 *= la[h];
               }
+              f0 = (f0 + bv0) * gelu_sig(g0 + bg0);
+              f1 = (f1 + bv1) * gelu_sig(g1 + bg1);
             } else {
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-            }
-          }
-          if (s == nsub - 1) {              // accumulator fully read: hand the stage back to the MMA warp before the stores
-            tc_fence_before();
-            if (PAIR) mbar_arrive_cluster(tempty_arrive);
-            else mbar_arrive(tempty_bar(acc));
-          }
-          if (HAS_RES && !RESST && s + 1 < nsub) load_res(s + 1, rnxt);
-          if (!GEGLU) {
-            if (LN) {                         // rstd * acc + (-mean rstd) * u + c in two FMAs per element
-              const uint32_t up = u_stage + s * EPI_COLS * 4, bp = bias_stage + s * EPI_COLS * 4;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 u4 = lds_f4(up + j * 4), b = lds_f4(bp + j * 4);
-                f[j] = fmaf(la, f[j], fmaf(lb, u4.x, b.x)); f[j + 1] = fmaf(la, f[j + 1], fmaf(lb, u4.y, b.y));
-                f[j + 2] = fmaf(la, f[j + 2], fmaf(lb, u4.z, b.z)); f[j + 3] = fmaf(la, f[j + 3], fmaf(lb, u4.w, b.w));
+              if (LN) {                         // rstd * acc + (-mean rstd) * u + c in two FMAs per element
+                f0 = fmaf(la[h], f0, fmaf(lb[h], u.x, b.x));
+                f1 = fmaf(la[h], f1, fmaf(lb[h], u.y, b.y));
+              } else if (has_bias) {
+                f0 += b.x; f1 += b.y;
               }
-            } else if (stage_bias) {
-              const uint32_t bp = bias_stage + s * EPI_COLS * 4;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 b = lds_f4(bp + j * 4);
-                f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
+              if (HAS_RV && rv[h] != nullptr) {
+                const float2 r2 = __ldg(reinterpret_cast<const float2*>(rv[h] + c));
+                f0 += r2.x; f1 += r2.y;
               }
             }
-            if (HAS_RV && rv && !rv_uniform) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 b = __ldg(reinterpret_cast<const float4*>(rv + s * EPI_COLS + j));
-                f[j] += b.x; f[j + 1] += b.y; f[j + 2] += b.z; f[j + 3] += b.w;
-              }
-            }
-          }
-          // thread = row -> lanes along columns: transpose this warp's 32 x 32 block through its own staging buffer.
-          // TMA stores were tried first: they queue behind the producer's prefetched loads in the same engine and their
-          // completion wait serialised the epilogue.
-          __syncwarp();                       // the previous sub-tile's readers of the staging buffer are done
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              const __half2 h = __floats2half2_rn(f[c * 8 + 2 * u], f[c * 8 + 2 * u + 1]);
-              pk[u] = *reinterpret_cast<const uint32_t*>(&h);
-            }
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(out_stage + sw64_off(lane, c)), "r"(pk[0]), "r"(pk[1]),
-                         "r"(pk[2]), "r"(pk[3]) : "memory");
-          }
-          __syncwarp();
-          if (RESST) cp_async_wait<MAXSUB_T - 1>();   // this lane's residual chunks of sub-tile s have landed
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {       // 8 rows x 64 contiguous bytes per store instruction
-            uint4 o;
-            asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
-                         : "r"(out_stage + sw64_off(i * 8 + tr, tch)));
-            if (HAS_RES) {                    // fp16 add: the rounding order of the reference's `linear(x) + residual`
-              __half2* oh = reinterpret_cast<__half2*>(&o);
-              uint4 rr;
-              if (RESST) {
-                asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(rr.x), "=r"(rr.y), "=r"(rr.z), "=r"(rr.w)
-                             : "r"(res_lane + (uint32_t)(i * 8 * C::RES_ROW_BYTES + s * 64)));
-              } else {
-                rr = rcur[i];
-              }
-              const __half2* rh = reinterpret_cast<const __half2*>(&rr);
-#pragma unroll
-              for (int u = 0; u < 4; ++u) oh[u] = __hadd2(oh[u], rh[u]);
-            }
-            if (tpix[i] >= 0) *reinterpret_cast<uint4*>(orow[i] + s * EPI_COLS) = o;
-            if (LNOUT) {                      // off the store's critical path: 8 values of row i*8+tr
-              const __half2* oh = reinterpret_cast<const __half2*>(&o);
-              const float2 a = __half22float2(oh[0]), b = __half22float2(oh[1]), c = __half22float2(oh[2]), d = __half22float2(oh[3]);
-              rs[i] += ((a.x + a.y) + (b.x + b.y)) + ((c.x + c.y) + (d.x + d.y));
-              float q0 = fmaf(a.x, a.x, a.y * a.y), q1 = fmaf(b.x, b.x, b.y * b.y);
-              float q2 = fmaf(c.x, c.x, c.y * c.y), q3 = fmaf(d.x, d.x, d.y * d.y);
-              rq[i] += (q0 + q1) + (q2 + q3);
-            }
-          }
-          if (RESST) stage_residual(s);       // the chunks just consumed are refilled with the next tile's rows
-        };
-#pragma unroll 1
-        for (int s = 0; s < nsub; s += 2) {
-          subtile(s, res_a, res_b);
-          if (s + 1 < nsub) subtile(s + 1, res_b, res_a);
-        }
-        if (RESST) {
-#pragma unroll 1
-          for (int s = nsub; s < MAXSUB_T; ++s) stage_residual(s);   // keep the group count per tile constant
-        }
-        if (LNOUT) {                          // the 4 column chunks of a row sit in 4 adjacent lanes
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            rs[i] += __shfl_xor_sync(0xffffffffu, rs[i], 1); rq[i] += __shfl_xor_sync(0xffffffffu, rq[i], 1);
-            rs[i] += __shfl_xor_sync(0xffffffffu, rs[i], 2); rq[i] += __shfl_xor_sync(0xffffffffu, rq[i], 2);
-            if (tch == 0 && tpix[i] >= 0) p.ln_sums_out[(long long)n_tile * p.M + tpix[i]] = make_float2(rs[i], rq[i]);
+            const __half2 hv = __floats2half2_rn(f0, f1);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(stage_buf + sw64_off((lane >> 2) + 8 * h, jj) + 4 * q),
+                         "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
           }
         }
-      } else {
-        // ------------------------------------------------------------ direct stores (tiny / unaligned N, linear only)
-        mbar_wait(tfull_bar(acc), aph);
-        tc_fence_after();
-        const float* rv = (p.rowvec != nullptr && pix >= 0) ? p.rowvec + (long long)(pix / p.pix_per_batch) * p.ldrv : nullptr;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 16) {
-          if (n0 + c0 >= p.N) break;   // warp-uniform
-          uint32_t v[16];
-          tmem_ld16(taddr + c0, v);
-          tmem_ld_wait();
-          if (pix < 0) continue;
-          __half* orow = p.out + (long long)pix * p.ldc;
-          const __half* rrow = p.residual ? p.residual + (long long)pix * p.ldr : nullptr;
-          const int n = n0 + c0;
+        __syncwarp();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (n + j < p.N) {
-              float f = __uint_as_float(v[j]);
-              if (has_bias) f += p.bias[n + j];
-              if (rv) f += rv[n + j];
-              if (rrow) f += __half2float(rrow[n + j]);
-              orow[n + j] = __float2half_rn(f);
-            }
+        for (int h = 0; h < 2; ++h) {           // 8 rows x 64 contiguous bytes per store instruction
+          uint4 o;
+          asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                       : "r"(stage_buf + sw64_off((lane >> 2) + 8 * h, q)));
+          if (HAS_RES) {                        // fp16 add: the rounding order of the reference's `linear(x) + residual`
+            __half2* oh = reinterpret_cast<__half2*>(&o);
+            const __half2* rh = reinterpret_cast<const __half2*>(&rr[h]);
+#pragma unroll
+            for (int t = 0; t < 4; ++t) oh[t] = __hadd2(oh[t], rh[t]);
+          }
+          if (pix[h] >= 0) *reinterpret_cast<uint4*>(orow[h] + sb * EPI_COLS) = o;
+          if (LNOUT) {
+            const __half2* oh = reinterpret_cast<const __half2*>(&o);
+            const float2 a = __half22float2(oh[0]), b2 = __half22float2(oh[1]), c2 = __half22float2(oh[2]), d2 = __half22float2(oh[3]);
+            rs[h] += ((a.x + a.y) + (b2.x + b2.y)) + ((c2.x + c2.y) + (d2.x + d2.y));
+            float q0 = fmaf(a.x, a.x, a.y * a.y), q1 = fmaf(b2.x, b2.x, b2.y * b2.y);
+            float q2 = fmaf(c2.x, c2.x, c2.y * c2.y), q3 = fmaf(d2.x, d2.x, d2.y * d2.y);
+            rq[h] += (q0 + q1) + (q2 + q3);
           }
         }
-        tc_fence_before();
-        if (PAIR) mbar_arrive_cluster(tempty_arrive);
-        else mbar_arrive(tempty_bar(acc));
+        __syncwarp();                           // staging buffer free for the next sub-tile
+      }
+      if (LNOUT) {                              // the 4 column chunks of a row sit in 4 adjacent lanes
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 1); rq[h] += __shfl_xor_sync(0xffffffffu, rq[h], 1);
+          rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 2); rq[h] += __shfl_xor_sync(0xffffffffu, rq[h], 2);
+          if (q == 0 && pix[h] >= 0) p.ln_sums_out[(long long)n_tile * p.M + pix[h]] = make_float2(rs[h], rq[h]);
+        }
+      }
+    } else {
+      // -------------------------------------------------------------- direct stores (tiny / unaligned N, linear only)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int h = e >> 1, c = 8 * j + 2 * q + (e & 1), n = n0 + c;
+          if (n < p.N && pix[h] >= 0) {
+            float f = acc[4 * j + e];
+            if (has_bias) f += p.bias[n];
+            if (rv[h]) f += rv[h][c];
+            if (p.residual) f += __half2float(p.residual[(long long)pix[h] * p.ldr + n]);
+            p.out[(long long)pix[h] * p.ldc + n] = __float2half_rn(f);
+          }
+        }
       }
     }
-    if (RESST) cp_async_wait<0>();             // only empty groups can be left; nothing in flight when the CTA exits
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();                  // nobody leaves while its peer may still signal it or read its smem
-  if (warp == 2) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, C::TMEM_COLS);
-    else tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 
@@ -668,57 +399,39 @@ ConvTile pick_conv_tile(int nimg, int H, int W) {
   return best;
 }
 
-template <int BN, int EPI, bool PAIR>
+template <int BN, int EPI>
 int launch(cudaStream_t st, const GemmParams& p) {
-  using C = Cfg<BN, PAIR, residual_staged(BN, EPI)>;
+  using C = Cfg<BN>;
   static bool configured = false;
   if (!configured) {
-    VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
-  if (PAIR) {
-    const int pairs = ((p.m_tiles + 1) / 2) * p.n_tiles;
-    const int max_clusters = num_sms() / 2;
-    return launch_pdl(gemm_tc_kernel<BN, EPI, PAIR>, dim3(2 * (pairs < max_clusters ? pairs : max_clusters)), dim3(GEMM_THREADS),
-                      C::SMEM_BYTES, st, 2, p);
-  }
   const int total = p.m_tiles * p.n_tiles;
-  return launch_pdl(gemm_tc_kernel<BN, EPI, PAIR>, dim3(total < num_sms() ? total : num_sms()), dim3(GEMM_THREADS), C::SMEM_BYTES,
+  return launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(total < num_sms() ? total : num_sms()), dim3(GEMM_THREADS), C::SMEM_BYTES,
                     st, 1, p);
 }
 
-template <int BN, bool PAIR>
+template <int BN>
 int launch_linear(cudaStream_t st, const GemmParams& p) {
-  int epi = (p.residual ? EPI_F_RES : 0) | (p.rowvec ? EPI_F_RV : 0) | ((p.ln_stats || p.ln_parts) ? EPI_F_LN : 0) |
-            (p.ln_sums_out ? EPI_F_LNOUT : 0);
-  // Whole-tile residual stage in shared memory: pays only where the epilogue, not the main loop, sets the tile time AND a
-  // 3-stage operand ring is deep enough -- measured: K = 320 (5 k-blocks) at M = 131072 -8 %; K = 640 +7 %, K = 1280 +20 %,
-  // CTA pairs +15 % (profiles/r02_resst_shapes.json).  So: single-CTA linear layers with K <= 320 only.
-  if constexpr (BN <= 160 && !PAIR) {
-    if ((epi == EPI_F_RES || epi == (EPI_F_LNOUT | EPI_F_RES)) && p.res_stage != 0 && p.staged != 0 && p.a_rank != 4 && p.num_kb <= 5)
-      epi |= EPI_F_RESST;
-    switch (epi) {
-      case EPI_F_RES | EPI_F_RESST: return launch<BN, EPI_F_RES | EPI_F_RESST, PAIR>(st, p);
-      case EPI_F_LNOUT | EPI_F_RES | EPI_F_RESST: return launch<BN, EPI_F_LNOUT | EPI_F_RES | EPI_F_RESST, PAIR>(st, p);
-      default: break;
-    }
-  }
+  const int epi = (p.residual ? EPI_F_RES : 0) | (p.rowvec ? EPI_F_RV : 0) | ((p.ln_stats || p.ln_parts) ? EPI_F_LN : 0) |
+                  (p.ln_sums_out ? EPI_F_LNOUT : 0);
   switch (epi) {
-    case EPI_F_LNOUT: return launch<BN, EPI_F_LNOUT, PAIR>(st, p);
-    case EPI_F_LNOUT | EPI_F_RES: return launch<BN, EPI_F_LNOUT | EPI_F_RES, PAIR>(st, p);
-    case EPI_F_LN: return launch<BN, EPI_F_LN, PAIR>(st, p);
-    case EPI_F_LN | EPI_F_RV: return launch<BN, EPI_F_LN | EPI_F_RV, PAIR>(st, p);
-    case 0: return launch<BN, 0, PAIR>(st, p);
-    case EPI_F_RES: return launch<BN, EPI_F_RES, PAIR>(st, p);
-    case EPI_F_RV: return launch<BN, EPI_F_RV, PAIR>(st, p);
-    case EPI_F_RES | EPI_F_RV: return launch<BN, EPI_F_RES | EPI_F_RV, PAIR>(st, p);
+    case EPI_F_LNOUT: return launch<BN, EPI_F_LNOUT>(st, p);
+    case EPI_F_LNOUT | EPI_F_RES: return launch<BN, EPI_F_LNOUT | EPI_F_RES>(st, p);
+    case EPI_F_LN: return launch<BN, EPI_F_LN>(st, p);
+    case EPI_F_LN | EPI_F_RV: return launch<BN, EPI_F_LN | EPI_F_RV>(st, p);
+    case 0: return launch<BN, 0>(st, p);
+    case EPI_F_RES: return launch<BN, EPI_F_RES>(st, p);
+    case EPI_F_RV: return launch<BN, EPI_F_RV>(st, p);
+    case EPI_F_RES | EPI_F_RV: return launch<BN, EPI_F_RES | EPI_F_RV>(st, p);
     default: set_error("gemm_tc: unsupported epilogue combination 0x%x", epi); return 2;
   }
 }
 
-// BLOCK_N by a two-term model: waves of the persistent grid x L2 -> SM bytes per k-block of one tile (the operand feed,
-// not the tensor pipe, bounds the main loop; see the file header).  Ties go to the wider tile only for long K, where
-// the main loop -- not the epilogue -- dominates.
+// BLOCK_N by a two-term model: waves of the persistent grid x shared-memory operand bytes per k-block of one tile
+// (16 KB of A + BN * 128 B of B; wider tiles need fewer bytes per flop).  Ties go to the wider tile only for long K,
+// where the main loop -- not the epilogue -- dominates.
 int pick_bn(int m_tiles, int N, int num_kb) {
   if (N <= 64) return 64;
   int best = 128;
@@ -788,9 +501,6 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   p.out = a.out;
   p.ldc = a.ldc;
   p.stages = get_option("gemm_stages");
-  p.epi_prefetch = get_option("epi_prefetch");
-  p.res_prefetch = get_option("res_prefetch");
-  p.res_stage = get_option("res_stage");
 
   if (a.taps != 1) {
     VS_REQUIRE(a.nimg > 0 && a.H > 0 && a.W > 0 && a.M == a.nimg * a.H * a.W, "gemm_tc: bad conv geometry");
@@ -847,15 +557,10 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   }
   VS_REQUIRE(bn == 64 || bn == 128 || bn == 160 || bn == 256, "gemm_tc: unsupported BLOCK_N %d", bn);
   p.n_tiles = (a.N + bn - 1) / bn;
-  // CTA pairs (cta_group::2) where the main loop dominates (K >= 768): measured -5..-13% there, but +5..+12% on the
-  // epilogue-bound K <= 640 shapes (two CTAs in lockstep, remote barrier arrivals).  "gemm_pair": 0 = never (A/B
-  // switch), 2 = whenever there are two row tiles.
-  const int pair_opt = get_option("gemm_pair");
-  const bool pair = pair_opt != 0 && p.m_tiles >= 2 && bn >= 128 && (p.num_kb >= 12 || pair_opt == 2);
   {
     const uint64_t dims[2] = {(uint64_t)Ktot, (uint64_t)a.N};
     const uint64_t str[1] = {(uint64_t)Ktot * 2};
-    const uint32_t box[2] = {BK, (uint32_t)(pair ? bn / 2 : bn)};   // a CTA pair: each CTA fetches half of the weight tile
+    const uint32_t box[2] = {BK, (uint32_t)bn};
     if (make_tmap_f16(&p.tmB, a.Bw, 2, dims, str, box, 1)) return 3;
   }
   // staged (transposed, coalesced) epilogue whenever the output geometry allows it: 16-byte strides, whole 32-column
@@ -870,21 +575,14 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   if (a.ln_sums_out) VS_REQUIRE(p.staged, "gemm_tc: row statistics output needs the staged epilogue (N %% 32 == 0, aligned rows)");
   ProfScope prof(st, a.taps != 1 ? PC_CONV : PC_GEMM, 2.0 * a.M * (double)a.N * Ktot, 1, a.M, a.N, Ktot);
   if (a.mode == EPI_GEGLU) {
-    if (p.ln_stats || p.ln_parts) return pair ? launch<256, EPI_F_GEGLU | EPI_F_LN, true>(st, p) : launch<256, EPI_F_GEGLU | EPI_F_LN, false>(st, p);
-    return pair ? launch<256, EPI_F_GEGLU, true>(st, p) : launch<256, EPI_F_GEGLU, false>(st, p);
-  }
-  if (pair) {
-    switch (bn) {
-      case 128: return launch_linear<128, true>(st, p);
-      case 256: return launch_linear<256, true>(st, p);
-      default: return launch_linear<160, true>(st, p);
-    }
+    if (p.ln_stats || p.ln_parts) return launch<256, EPI_F_GEGLU | EPI_F_LN>(st, p);
+    return launch<256, EPI_F_GEGLU>(st, p);
   }
   switch (bn) {
-    case 64: return launch_linear<64, false>(st, p);
-    case 128: return launch_linear<128, false>(st, p);
-    case 256: return launch_linear<256, false>(st, p);
-    default: return launch_linear<160, false>(st, p);
+    case 64: return launch_linear<64>(st, p);
+    case 128: return launch_linear<128>(st, p);
+    case 256: return launch_linear<256>(st, p);
+    default: return launch_linear<160>(st, p);
   }
 }
 

@@ -1,4 +1,4 @@
-// Host-side launchers of the sm_100a kernels (all asynchronous on `st`, no hidden allocation, return 0 on success).
+// Host-side launchers of the sm_90a kernels (all asynchronous on `st`, no hidden allocation, return 0 on success).
 // Activation layout everywhere: NHWC fp16, i.e. tokens [(b f), h*w, C] with C innermost.
 #pragma once
 #include <cuda_fp16.h>
@@ -75,7 +75,7 @@ int ln_fold(cudaStream_t st, const __half* w, int N, int K, const float* gamma, 
 int attention(cudaStream_t st, const __half* q, int ldq, const __half* k, int ldk, const __half* v, int ldv,
               __half* o, int ldo, int batch, int nq, int nk, int heads, int d, long long q_bstride,
               long long kv_bstride, long long o_bstride, int kv_div);   // k/v batch index = batch / kv_div
-// tcgen05/TMEM implementation (d = 40, 80); returns -1 if the shape is not supported by it.
+// wgmma/TMA implementation (d = 40, 80); returns -1 if the shape is not supported by it.
 int attention_tc(cudaStream_t st, const __half* q, int ldq, const __half* k, int ldk, const __half* v, int ldv,
                  __half* o, int ldo, int batch, int nq, int nk, int heads, int d, long long q_bstride,
                  long long kv_bstride, long long o_bstride, int kv_div);
@@ -85,8 +85,7 @@ int attention_probs(cudaStream_t st, const __half* q, int ldq, const __half* k, 
                     int heads, int d, long long q_bstride, long long kv_bstride, int kv_div);
 int attention_apply_probs(cudaStream_t st, const __half* probs, const __half* v, int ldv, __half* o, int ldo, int batch, int nq,
                           int nk, int heads, int d, long long kv_bstride, long long o_bstride, int kv_div);
-int attention_debug_read(unsigned long long* host, int n);   // counters of the "attn_debug" kernels (148 x 8)
-// runtime options: "attn_tc" (1 = use the tcgen05 attention kernel where supported, default 1)
+// runtime options: "attn_tc" (1 = use the wgmma attention kernel where supported, default 1)
 int set_option(const char* name, int value);
 int get_option(const char* name);
 // Temporal attention across F frames per pixel: qkv [B, F, HW, 3C] -> o [B, F, HW, C].
@@ -98,7 +97,7 @@ int small_linear(cudaStream_t st, const float* x, int rows, int K, const __half*
 int timestep_embedding(cudaStream_t st, const float* t, int B, int dim, float* out);   // cat(cos, sin)
 int conv_in_3x3(cudaStream_t st, const __half* x, int nimg, int H, int W, int cin, const __half* w, const float* bias,
                 int cout, __half* out, __half* scratch = nullptr);   // conv_in (tiny Cin): with `scratch` (>= (nimg*H*W +
-                // cout) * 64 halves, cin == 4) patch rows + tcgen05 GEMM, else a direct CUDA-core kernel
+                // cout) * 64 halves, cin == 4) patch rows + tensor-core GEMM, else a direct CUDA-core kernel
 int upsample_nearest2x(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out);
 int im2col_s2(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out);  // [nimg*Ho*Wo, 9*C]
 int add_inplace(cudaStream_t st, __half* x, const __half* r, size_t n, float scale);   // x += scale * r

@@ -500,11 +500,9 @@ int groupnorm_frame_fused(cudaStream_t st, const __half* x, int C, int nimg, int
   int ncta = 1;
   while ((img_bytes + ncta - 1) / ncta > cap && ncta < 16) ncta *= 2;
   if ((img_bytes + ncta - 1) / ncta > cap || hw % ncta != 0) return -1;
-  // Measured (profiles/r02_bench_gn_fused_ab.json): images of <= 4 CTAs (the 16x16 / 8x8 levels) 19 us vs 30 us for the
-  // statistics + apply pair; 8- and 16-CTA clusters (32x32 / 64x64) are SLOWER (44 vs 42 us, 80 vs 68 us): one 164 KB CTA per
-  // SM with a barrier between its read and its write phase keeps too few bytes in flight, and 16-CTA clusters leave 20 of the
-  // 148 SMs idle.  "gn_fused" = 1 therefore takes the single pass only up to 4 CTAs; 2 = always (A/B).
-  if (ncta > 4 && get_option("gn_fused") != 2) return -1;
+  // Measured on an H100 80GB HBM3 (400 W power limit), 32 images, single pass vs statistics + apply pair: 64x64x320 (16 CTAs)
+  // 91.5 vs 103.6 us, 32x32x640 (8) 49.4 vs 58.9 us, 16x16x1280 (4) 28.1 vs 24.6 us, 8x8x1280 (1) 19.5 vs 23.7 us.  The single
+  // pass wins at three of the four levels and in sum, so every cluster size takes it ("gn_fused" != 0).
   const int ppc = hw / ncta;
   const size_t smem = 512 + (size_t)ppc * C * 2;
   static bool configured = false;

@@ -96,8 +96,8 @@ __global__ void conv_in_kernel(const __half* __restrict__ x, int nimg, int H, in
 }
 
 // conv_in on the tensor cores: the 36-wide patch of every pixel (9 taps x 4 channels, zero padded to one 64-column
-// k-block) is written once as an fp16 row, the weight goes to [cout][64] in the same order, and the tcgen05 GEMM does the
-// rest (the direct kernel above took 1.37 ms of the 55 ms step; this path takes ~0.06 ms).
+// k-block) is written once as an fp16 row, the weight goes to [cout][64] in the same order, and the wgmma GEMM does the
+// rest (the direct kernel above reads the 4-channel input once per output channel block and is much slower).
 __global__ void conv_in_patch_kernel(const __half* __restrict__ x, int nimg, int H, int W, uint4* __restrict__ out) {
   const long long total = (long long)nimg * H * W * 8;   // eight 16-byte chunks (two taps each) per pixel
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {

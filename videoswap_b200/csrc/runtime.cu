@@ -73,7 +73,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -115,18 +115,7 @@ ProfScope::~ProfScope() {
 // A/B switches of the kernels (name, value).  Defaults are the shipped configuration.
 struct Option { const char* name; int value; };
 static Option g_options[] = {
-    {"attn_tc", 1},        // tcgen05 attention for d = 40 / 80 (0 = mma.sync kernel)
-    {"attn_persist", 1},   // persistent tcgen05 attention with two issuer warps (0 = round-1 kernel: one CTA per item, one issuer)
-    {"attn_epiwg", 1},     // persistent d = 40 attention: dedicated epilogue warpgroup + double-buffered O accumulators
-    {"attn_pingpong", 1},  // persistent attention: MUFU ping-pong of the two softmax warpgroups (0 = free-running, A/B)
-    {"attn_ptmem", 1},     // persistent attention: P handed to the P V MMA through tensor memory instead of shared memory
-    {"attn_debug", 0},     // 1: persistent d = 40 attention records per-CTA cycle counters (vs_debug_read)
-    {"attn_poly", 1},      // P chunks (of 8 per key tile) whose exp2 runs on the FMA pipe instead of MUFU (0..3)
-    {"attn_handoff", 1},   // 1: the softmax ping-pong hands the MUFU pipe over after 7 of 8 key chunks, 0: after the last
-    {"gemm_pair", 1},      // CTA pairs (cta_group::2, 256-row tiles): 1 = for K >= 768, 0 = never, 2 = whenever possible
-    {"res_stage", 1},      // linear layers with a residual, K <= 320: residual tile staged in shared memory a whole tile ahead
-    {"res_prefetch", 0},   // GEMM epilogue: residual rows of the next tile prefetched into L2 (1 = per 128 B, 2 = bulk per row)
-    {"epi_prefetch", 0},   // GEMM epilogue: TMEM load of sub-tile s+1 issued while sub-tile s is processed (A/B)
+    {"attn_tc", 1},        // wgmma attention for d = 40 / 80 (0 = mma.sync kernel)
     {"gemm_stages", 0},    // smem ring depth limit (0 = all)
     {"ln_fold", 1},        // LayerNorms folded into the GEMM that consumes them (0 = stand-alone LayerNorm kernel)
     {"ln_fuse", 1},        // row statistics of folded LayerNorms come from the producing GEMM's epilogue (0 = ln_stats_kernel pass)

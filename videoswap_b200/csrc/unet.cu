@@ -1,5 +1,5 @@
 // Host-side executor of the reference's AnimateDiffUNet3DModel.forward (videoswap/models/animatediff_models/unet.py:
-// 328-481 and unet_blocks.py) on top of the sm_100a kernels.  Owns the packed weights and a static activation
+// 328-481 and unet_blocks.py) on top of the sm_90a kernels.  Owns the packed weights and a static activation
 // workspace; activations are NHWC fp16 ([(b f), h*w, C] tokens), so none of the reference's rearrange/permute/concat
 // copies exist.  Weight names are the reference's state_dict keys.
 #include <math.h>

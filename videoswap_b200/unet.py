@@ -6,7 +6,7 @@ What is mirrored (SURVEY.md 8b.1): constructor arguments / `.config`, the module
 `to_q`..., `load_state_dict` (weights are re-packed into kernel layouts on the next forward), the `forward` signature,
 in-place `pop(0)` consumption of `down_block_additional_residuals`, `UNet3DConditionOutput`.
 
-The torch modules below are parameter HOLDERS only: all arithmetic happens in the sm_100a kernels.  There is no
+The torch modules below are parameter HOLDERS only: all arithmetic happens in the sm_90a kernels.  There is no
 PyTorch/CPU fallback; a missing shared library or a CPU tensor raises.
 """
 from __future__ import annotations
