@@ -110,17 +110,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug must trap (-> CUDA error at the next sync) instead of hanging the GPU box.
+// Bounded wait: a pipeline bug must trap (-> CUDA error at the next sync) instead of hanging the GPU.
+// No printf here: a call anywhere in a kernel makes ptxas serialise every wgmma of that kernel (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   // try_wait suspends the thread in hardware for a bounded time, so this loop iterates every ~100 cycles; the watchdog
   // counts iterations (2^25 of them is seconds) instead of reading the clock on the hot path
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 25)) {
-      printf("vs: mbarrier wait timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (++spins > (1u << 25)) __trap();
   }
 }
 
@@ -230,15 +228,36 @@ __device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t da, uint64_t db,
       : VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24)
       : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
 }
-template <int TB = 0>
-__device__ __forceinline__ void wgmma_m64n32(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, %19;\n\t}"
-      : VS_R8(0), VS_R8(8)
-      : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
-}
+// m64nNk16 with both operands K-major in shared memory: one instruction for the full width of a GEMM tile (N / 2
+// accumulators per thread, in the register layout of wgmma_m64n64 extended to N columns).
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t scale_d);
+#define VS_REGS_0_31 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+#define VS_REGS_32_63 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+#define VS_REGS_64_79 "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79"
+#define VS_REGS_80_127 "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+// N, accumulator operand list, operand numbers of da / db / scale_d (= N / 2 ...), accumulator constraints
+#define VS_WGMMA_SS(N, REGS, IA, IB, IS, ...)                                                                     \
+  template <>                                                                                                     \
+  __device__ __forceinline__ void wgmma_ss<N>(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {           \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #IS ", 0;\n\t"                                         \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 {" REGS "}, %" #IA ", %" #IB ", p, 1, 1, 0, 0;\n\t}" \
+                 : __VA_ARGS__                                                                                    \
+                 : "l"(da), "l"(db), "r"(scale_d));                                                               \
+  }
+VS_WGMMA_SS(64, VS_REGS_0_31, 32, 33, 34, VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24))
+VS_WGMMA_SS(128, VS_REGS_0_31 "," VS_REGS_32_63, 64, 65, 66, VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24), VS_R8(32), VS_R8(40),
+            VS_R8(48), VS_R8(56))
+VS_WGMMA_SS(160, VS_REGS_0_31 "," VS_REGS_32_63 "," VS_REGS_64_79, 80, 81, 82, VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24),
+            VS_R8(32), VS_R8(40), VS_R8(48), VS_R8(56), VS_R8(64), VS_R8(72))
+VS_WGMMA_SS(256, VS_REGS_0_31 "," VS_REGS_32_63 "," VS_REGS_64_79 "," VS_REGS_80_127, 128, 129, 130, VS_R8(0), VS_R8(8),
+            VS_R8(16), VS_R8(24), VS_R8(32), VS_R8(40), VS_R8(48), VS_R8(56), VS_R8(64), VS_R8(72), VS_R8(80), VS_R8(88),
+            VS_R8(96), VS_R8(104), VS_R8(112), VS_R8(120))
+#undef VS_WGMMA_SS
+#undef VS_REGS_0_31
+#undef VS_REGS_32_63
+#undef VS_REGS_64_79
+#undef VS_REGS_80_127
 template <int TB = 0>
 __device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(

@@ -2,10 +2,13 @@
 //
 // One persistent, warp-specialised kernel of three warpgroups: warpgroup 0 is the TMA producer (one elected thread of
 // warp 0 issues the copies; the warpgroup gives most of its registers to the others with setmaxnreg), warpgroups 1 and 2
-// are the consumers: each owns 64 rows of the 128 (M) x BN (N) tile, issues wgmma.m64nNk16 on the 128-byte-swizzled
-// operand ring in shared memory and keeps its accumulator in registers.  K advances 64 elements (one swizzle row of
-// fp16) per ring stage; the producer runs up to STAGES k-blocks ahead, across tile boundaries, so the next tile's
-// operands are in flight while the consumers run the epilogue of the current one.
+// are ping-pong consumers.  A tile is 64 (M) x BN (N); the tiles of a CTA alternate between the two consumers, each of
+// which issues one full-width wgmma.m64nBNk16 per k16 step on the 128-byte-swizzled operand ring in shared memory and
+// keeps its accumulator in registers.  Two named barriers hand the tensor cores from one consumer to the other once its
+// MMAs are issued, so one consumer's epilogue runs under the other's main loop.  A CTA walks 128-row x BN units whose
+// two 64-row halves go to the two consumers back to back: the second load of the weight tile hits L2.  K advances 64
+// elements (one swizzle row of fp16) per ring stage; the producer fills the ring in the order the consumers take the
+// tiles and runs up to STAGES k-blocks ahead, across tile boundaries.
 // A 3x3 convolution is the same kernel with nine K segments: tap (dy,dx) loads the NHWC activation box shifted by
 // (dy,dx) through a 4-D TMA descriptor and the out-of-bounds zero fill of TMA provides the padding; a channel concat
 // is two descriptors walked back to back along K.
@@ -24,9 +27,9 @@ namespace vs {
 
 namespace {
 
-constexpr int BM = 128;
+constexpr int BM = 64;                              // rows of a tile (= of one consumer warpgroup)
 constexpr int BK = 64;
-constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
+constexpr int A_STAGE_BYTES = BM * BK * 2;          // 8 KB
 constexpr int GEMM_THREADS = 384;                   // producer warpgroup + 2 consumer warpgroups
 constexpr int SMEM_LIMIT = 227 * 1024;
 constexpr int EPI_COLS = 32;                        // output columns per epilogue sub-tile (64 B of fp16)
@@ -72,7 +75,7 @@ struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
+  static constexpr int STAGES = STAGES_RAW > 12 ? 12 : STAGES_RAW;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(B_STAGE_BYTES % 1024 == 0, "B stage must keep 1024-byte alignment for SWIZZLE_128B");
   static_assert(STAGES >= 3, "pipeline too shallow");
@@ -81,14 +84,6 @@ struct Cfg {
 
 __device__ __forceinline__ uint32_t sw64_off(int row, int chunk) {   // byte offset inside a [rows x 64 B] swizzled tile
   return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4));
-}
-
-// acc (+)= A[64 rows] B[BN rows]^T over one k16 step: BN / 64 m64n64 instructions and one m64n32 for the rest.
-template <int BN>
-__device__ __forceinline__ void mma_k16(float* acc, uint64_t da, uint64_t db, uint32_t scale_d) {
-#pragma unroll
-  for (int c = 0; c < BN / 64; ++c) wgmma_m64n64(acc + 32 * c, da, db + (uint64_t)(c * 64 * 128 / 16), scale_d);
-  if (BN % 64) wgmma_m64n32(acc + 32 * (BN / 64), da, db + (uint64_t)((BN / 64) * 64 * 128 / 16), scale_d);
 }
 
 template <int BN, int EPI>
@@ -114,11 +109,16 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
-  const int total_tiles = p.m_tiles * p.n_tiles;
   const int nst = (p.stages > 0 && p.stages < C::STAGES) ? p.stages : C::STAGES;   // ring depth (debug knob: "gemm_stages")
-  // Tile order: n fastest, tiles round-robin over the CTAs (CTAs running at the same time share the A row panel and a
-  // few weight tiles in L2).
-  const int t_begin = blockIdx.x, t_step = gridDim.x;
+  // Tile order: units of (two 64-row tiles) x (one column tile), n fastest, round-robin over the CTAs (CTAs running at
+  // the same time share the A row panel and a few weight tiles in L2); the halves of a unit are consecutive tiles of the
+  // CTA and so go to the two consumers.
+  const int total_units = ((p.m_tiles + 1) >> 1) * p.n_tiles;
+  auto next_tile = [&](int& u, int& h) {       // (unit u, half h) -> the CTA's next tile; u >= total_units at the end
+    if (h == 0 && 2 * (u / p.n_tiles) + 1 < p.m_tiles) { h = 1; return; }
+    h = 0;
+    u += gridDim.x;
+  };
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&p.tmA);
@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     if (p.kb_src1 < p.kb_per_tap) prefetch_tmap(&p.tmA2);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 8);                // one arrival per consumer warp
+      mbar_init(empty_bar(s), 4);                // one arrival per warp of the consumer that read the stage
     }
     fence_barrier_init();
   }
@@ -142,8 +142,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     const bool conv = p.a_rank == 4;
     const int tap_x0 = p.tap_x0, tap_x1 = p.tap_x0 + p.tap_w;
     uint32_t pr_s = 0, pr_ph = 0;              // ring stage / phase, carried across tiles
-    for (int tile = t_begin; tile < total_tiles; tile += t_step) {
-      const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
+    for (int u = blockIdx.x, h = 0; u < total_units; next_tile(u, h)) {
+      const int m_tile = 2 * (u / p.n_tiles) + h, n_tile = u % p.n_tiles;
       int x0 = 0, y0 = 0, i0 = 0;
       if (conv) {
         x0 = (m_tile % p.tiles_x) * p.TW;
@@ -182,10 +182,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 
   // ===================================================================== consumers: MMA + epilogue
   setmaxnreg_inc<CONSUMER_REGS>();
-  const int g = wg - 1;                        // rows [64 g, 64 g + 64) of the tile
-  const int wq = warp & 3;                     // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of those
+  const int g = wg - 1;                        // consumer g takes the CTA's tiles j with j % 2 == g
+  const int wq = warp & 3;                     // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of the tile
   const int q = lane & 3;
-  const int rbase = 64 * g + 16 * wq + (lane >> 2);   // this thread's tile rows: rbase and rbase + 8
+  const int rbase = 16 * wq + (lane >> 2);     // this thread's tile rows: rbase and rbase + 8
   const uint32_t stage_buf = epi_base + (uint32_t)(warp - 4) * EPI_WARP_BYTES;
   const bool has_bias = p.bias != nullptr;
   const bool staged = p.staged != 0;
@@ -204,19 +204,31 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     return px < p.M ? px : -1;
   };
 
+  // Tensor-core hand-off: consumer g waits on named barrier 1 + g before its main loop and, once all MMAs of its tile are
+  // issued, arrives on the other consumer's barrier -- only when the CTA has a next tile, so every arrival is waited for.
+  const int bar_mine = 1 + g, bar_other = 2 - g;
   float acc[BN / 2];
-  uint32_t s = 0, ph = 0;
-  for (int tile = t_begin; tile < total_tiles; tile += t_step) {
+  uint32_t s = 0, ph = 0;                      // ring stage / phase of the next tile's first k-block
+  for (int u = blockIdx.x, h = 0, j = 0; u < total_units; ++j) {
+    const int m_tile = 2 * (u / p.n_tiles) + h, n_tile = u % p.n_tiles;
+    next_tile(u, h);
+    if ((j & 1) != g) {                        // the other consumer's tile: skip its k-blocks in the ring
+      const uint32_t t = s + (uint32_t)num_kb;
+      ph ^= (t / (uint32_t)nst) & 1u;
+      s = t % (uint32_t)nst;
+      continue;
+    }
     // ------------------------------------------------------------------ main loop
+    if (j > 0) named_bar_sync(bar_mine, 256);
     uint32_t prev = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(full_bar(s), ph);
       wgmma_fence();
       const uint32_t a_addr = smem_base + s * C::STAGE_BYTES;
-      const uint64_t da = gmma_desc_sw128(a_addr + g * 64 * 128);
+      const uint64_t da = gmma_desc_sw128(a_addr);
       const uint64_t db = gmma_desc_sw128(a_addr + A_STAGE_BYTES);
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) mma_k16<BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
       wgmma_commit();
       if (kb > 0) {                            // the MMAs of the previous k-block have read their stage: release it
         wgmma_wait<1>();
@@ -225,11 +237,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       prev = s;
       if (++s == (uint32_t)nst) { s = 0; ph ^= 1; }
     }
+    if (u < total_units) named_bar_arrive(bar_other, 256);
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(empty_bar(prev));
 
     // ------------------------------------------------------------------ epilogue
-    const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
     const int n0 = n_tile * BN;
     int pix[2];
     pix[0] = tile_pixel(m_tile, rbase);
@@ -382,12 +394,12 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 
 struct ConvTile { int tw, th, tn; };
 
-ConvTile pick_conv_tile(int nimg, int H, int W) {
-  ConvTile best{1, 1, 128};
+ConvTile pick_conv_tile(int nimg, int H, int W) {   // BM pixels as a TW x TH x TN box with the least padding
+  ConvTile best{1, 1, BM};
   long long best_cost = -1;
-  for (int tw = 1; tw <= 128; tw *= 2) {
-    for (int th = 1; tw * th <= 128; th *= 2) {
-      const int tn = 128 / (tw * th);
+  for (int tw = 1; tw <= BM; tw *= 2) {
+    for (int th = 1; tw * th <= BM; th *= 2) {
+      const int tn = BM / (tw * th);
       if (tw > 256 || th > 256 || tn > 256) continue;
       const long long cost = (long long)((W + tw - 1) / tw) * tw * ((H + th - 1) / th) * th * ((nimg + tn - 1) / tn) * tn;
       if (best_cost < 0 || cost < best_cost || (cost == best_cost && tw > best.tw)) {
@@ -407,7 +419,7 @@ int launch(cudaStream_t st, const GemmParams& p) {
     VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
-  const int total = p.m_tiles * p.n_tiles;
+  const int total = ((p.m_tiles + 1) / 2) * p.n_tiles;   // units of two tiles
   return launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(total < num_sms() ? total : num_sms()), dim3(GEMM_THREADS), C::SMEM_BYTES,
                     st, 1, p);
 }
@@ -429,10 +441,10 @@ int launch_linear(cudaStream_t st, const GemmParams& p) {
   }
 }
 
-// BLOCK_N by a two-term model: waves of the persistent grid x shared-memory operand bytes per k-block of one tile
-// (16 KB of A + BN * 128 B of B; wider tiles need fewer bytes per flop).  Ties go to the wider tile only for long K,
+// BLOCK_N by a two-term model: waves of the persistent grid x operand bytes per k-block of one unit of two tiles
+// (2 x 8 KB of A + BN * 128 B of B; wider tiles need fewer bytes per flop).  Ties go to the wider tile only for long K,
 // where the main loop -- not the epilogue -- dominates.
-int pick_bn(int m_tiles, int N, int num_kb) {
+int pick_bn(int m_units, int N, int num_kb) {
   if (N <= 64) return 64;
   int best = 128;
   long long best_cost = -1;
@@ -440,8 +452,8 @@ int pick_bn(int m_tiles, int N, int num_kb) {
   for (int i = 0; i < 3; ++i) {
     const int bn = cand[i];
     if (bn != 128 && N % bn != 0) continue;
-    const long long tiles = (long long)m_tiles * ((N + bn - 1) / bn);
-    const long long waves = (tiles + num_sms() - 1) / num_sms();
+    const long long units = (long long)m_units * ((N + bn - 1) / bn);
+    const long long waves = (units + num_sms() - 1) / num_sms();
     const long long cost = waves * (16 + bn / 8);           // KB per k-block: 16 (A) + bn * 128 B (B)
     if (best_cost < 0 || cost < best_cost || (cost == best_cost && num_kb >= 40)) {
       best_cost = cost;
@@ -460,7 +472,7 @@ int gemm_n_tiles(const GemmArgs& a) {
   if (a.taps != 1) return 0;
   int bn = a.force_bn;
   if (a.mode == EPI_GEGLU) bn = 2 * kGegluGranule;
-  else if (bn == 0) bn = pick_bn((a.M + BM - 1) / BM, a.N, (a.K1 + BK - 1) / BK + a.K2 / BK);
+  else if (bn == 0) bn = pick_bn((a.M + 2 * BM - 1) / (2 * BM), a.N, (a.K1 + BK - 1) / BK + a.K2 / BK);
   return (a.N + bn - 1) / bn;
 }
 
@@ -553,7 +565,7 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
     VS_REQUIRE(a.N % bn == 0, "gemm_tc: GEGLU needs N %% %d == 0 (N=%d)", bn, a.N);
     VS_REQUIRE(a.bias != nullptr && a.residual == nullptr && a.rowvec == nullptr, "gemm_tc: GEGLU takes a bias only");
   } else if (bn == 0) {
-    bn = pick_bn(p.m_tiles, a.N, p.num_kb);
+    bn = pick_bn((p.m_tiles + 1) / 2, a.N, p.num_kb);
   }
   VS_REQUIRE(bn == 64 || bn == 128 || bn == 160 || bn == 256, "gemm_tc: unsupported BLOCK_N %d", bn);
   p.n_tiles = (a.N + bn - 1) / bn;
