@@ -149,16 +149,48 @@ int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0, const voi
                      int h, int w, float rate, int coord_fp16, float scale, float* d_ws, void* d_map);
 
 /* ---- per-kernel entry points (used by the parity tests; same kernels the forward uses) -------------------------- */
-int vs_gemm(void* stream, const void* d_A, int K1, const void* d_A2, int K2, const void* d_W, int M, int N,
-            const float* d_bias, const float* d_rowvec, int pix_per_batch, const void* d_residual, void* d_out, int mode,
-            int force_bn);
-int vs_conv3x3(void* stream, const void* d_x, int C1, const void* d_x2, int C2, const void* d_w_packed, int nimg, int H,
-               int W, int Cout, const float* d_bias, const float* d_rowvec, int imgs_per_batch, const void* d_residual,
-               void* d_out);
+/* One launch of the tensor-core GEMM / implicit-GEMM convolution with every argument the UNet forward can pass (field for
+ * field the library's internal GEMM arguments; zero-initialise and set what is used).
+ *   out[pix, n] = epilogue( sum_k [A | A2][pix (+ tap shift), k] * Bw[n, k] )
+ *   taps 1: A [M, K1] (row stride lda1) (+ A2 [M, K2], lda2, channel concat along K); taps 9: NHWC [nimg, H, W, K1] 3x3
+ *   convolution, pad 1 (M = nimg H W); taps 4: one output parity (sub_py, sub_px) of nearest-2x + 3x3.  Bw [N, taps (K1 + K2)].
+ *   Epilogue: + bias[n] + rowvec[((pix / pix_per_batch) % rv_mod if rv_mod > 0), n] (row stride ldrv, 0 = N) + residual[pix, n]
+ *   (row stride ldr; may alias `out`); mode 1 = GEGLU on packed weights (N / 2 output columns).  Folded LayerNorm of A:
+ *   ln_u [N] with ln_stats [M, 2] (rstd, -mean rstd) or ln_parts [ln_nparts][M][2] (sum, sum of squares).
+ *   ln_sums_out [n_tiles][M][2]: (sum, sum of squares) of the stored fp16 outputs per row and column tile of width BN.
+ *   force_bn 0 = automatic column-tile width, else 64 / 128 / 160 / 256. */
+typedef struct vs_gemm_desc {
+  const void* A; int K1; int lda1;
+  const void* A2; int K2; int lda2;
+  const void* Bw;
+  int M, N;
+  int taps;
+  int sub_py, sub_px;
+  int nimg, H, W;
+  const float* bias;
+  const float* rowvec; int ldrv; int pix_per_batch; int rv_mod;
+  const float* ln_stats; const float* ln_u;
+  const float* ln_parts; int ln_nparts;
+  float* ln_sums_out;
+  const void* residual; int ldr;
+  void* out; int ldc;
+  int mode;
+  int force_bn;
+} vs_gemm_desc;
+int vs_gemm_ex(void* stream, const vs_gemm_desc* desc);
 int vs_pack_conv3x3(void* stream, const void* d_w, int cout, int cin, void* d_out);
 int vs_pack_geglu(void* stream, const void* d_w, const void* d_b, int hidden, int K, void* d_wout, float* d_bout);
 int vs_groupnorm(void* stream, const void* d_x1, int c1, const void* d_x2, int c2, int nimg, int hw, int imgs_per_set,
                  int groups, float eps, const float* d_gamma, const float* d_beta, int silu, float* d_sums, void* d_out);
+/* The two halves of the statistics + apply GroupNorm as the frame-sharded forward runs them: vs_groupnorm_stats ADDS the
+ * (sum, sum of squares) of each set of imgs_per_set images to d_sums [nimg / imgs_per_set, groups, 2] (zeroed first only
+ * when zero_first != 0); vs_groupnorm_apply normalises with sums that cover count_scale times the local elements (the
+ * all-reduced sums of count_scale frame shards). */
+int vs_groupnorm_stats(void* stream, const void* d_x1, int c1, const void* d_x2, int c2, int nimg, int hw, int imgs_per_set,
+                       int groups, float* d_sums, int zero_first);
+int vs_groupnorm_apply(void* stream, const void* d_x1, int c1, const void* d_x2, int c2, int nimg, int hw, int imgs_per_set,
+                       int groups, const float* d_sums, float eps, const float* d_gamma, const float* d_beta, int silu,
+                       int count_scale, void* d_out);
 int vs_layernorm(void* stream, const void* d_x, int rows, int C, const float* d_gamma, const float* d_beta,
                  const float* d_pe, int hw, int F, void* d_out);
 /* LayerNorm(x) (+ pe[(row / hw) % frames]) followed by a linear layer (mode 0) or GEGLU projection (mode 1, packed
@@ -171,17 +203,21 @@ int vs_ln_linear(void* stream, const void* d_x, int M, int C, const void* d_w, c
 /* The form the UNet forward uses: the linear layer that PRODUCES the LayerNorm's input (x = x0 W0^T + b0 (+ residual),
  * fp16, written to d_x) also emits the per-row (sum, sum of squares) of what it stores, one slice per column tile of its
  * epilogue (d_parts: [parts_capacity][M][2] fp32), and the consuming GEMM derives mean / rstd from those slices -- no
- * statistics pass over x (attention.py:229-256 / motion_module.py:224-234: proj_in -> norm1 -> to_q/k/v, ...). */
+ * statistics pass over x (attention.py:229-256 / motion_module.py:224-234: proj_in -> norm1 -> to_q/k/v, ...).
+ * d_pe / pe_len / hw / frames / d_cpe as in vs_ln_linear: the motion module's temporal positional encoding. */
 int vs_linear_ln_linear(void* stream, const void* d_x0, int M, int K0, const void* d_w0, const float* d_b0,
                         const void* d_residual, int C, void* d_x, const void* d_w, const float* d_bias, int N,
-                        const float* d_gamma, const float* d_beta, int mode, void* d_wf, float* d_u, float* d_c,
-                        float* d_parts, int parts_capacity, void* d_out);
+                        const float* d_gamma, const float* d_beta, const float* d_pe, int pe_len, int hw, int frames,
+                        int mode, void* d_wf, float* d_u, float* d_c, float* d_cpe, float* d_parts, int parts_capacity,
+                        void* d_out);
 int vs_attention(void* stream, const void* d_q, int ldq, const void* d_k, int ldk, const void* d_v, int ldv, void* d_o,
                  int ldo, int batch, int nq, int nk, int heads, int d, long long q_bstride, long long kv_bstride,
                  long long o_bstride, int kv_div);
 int vs_temporal_attention(void* stream, const void* d_qkv, void* d_o, int B, int F, int HW, int C, int heads);
+/* conv_in (3x3, pad 1, tiny cin).  With d_scratch (>= (nimg H W + cout) * 64 halves) and cin == 4: patch rows + the
+ * tensor-core GEMM with K = 64, as the UNet forward runs it; d_scratch NULL (or cin != 4): a direct CUDA-core kernel. */
 int vs_conv_in(void* stream, const void* d_x, int nimg, int H, int W, int cin, const void* d_w, const float* d_bias,
-               int cout, void* d_out);
+               int cout, void* d_scratch, void* d_out);
 int vs_upsample2x(void* stream, const void* d_x, int nimg, int H, int W, int C, void* d_out);
 /* Upsample3D (resnet.py:21-69): nearest 2x then conv3x3, computed as four 2x2 sub-pixel convolutions on the low-resolution
  * input (weights pre-summed per output parity; 2.25x fewer FLOPs, no materialised up-sampled tensor).  d_w: [Cout, C, 3, 3]
@@ -202,6 +238,8 @@ int vs_profile_dump(const char* path);   /* CSV: category, shape (m,n,k), work p
 /* Runtime A/B switches (defaults = the shipped configuration; unknown names are an error):
  *   "attn_tc"      1  wgmma/TMA attention kernel for head dims 40/80; 0 forces the mma.sync kernel
  *   "gemm_stages"  0  limit of the shared-memory ring depth of the GEMM (0 = as many as fit)
+ *   "gemm_ctas"    0  cap on the persistent grid of the GEMM (0 = one CTA per SM); a smaller grid gives every CTA more
+ *                     tiles, so the same problem runs another tile schedule (schedule-invariance tests)
  *   "ln_fold"      1  LayerNorms folded into the consuming GEMM; 0 = stand-alone LayerNorm kernel
  *   "ln_fuse"      1  row statistics of folded LayerNorms written by the producing GEMM's epilogue; 0 = ln_stats pass
  *   "tattn_vst"    1  temporal attention writes its outputs with 16-byte stores from a shared-memory stage; 0 = 4-byte stores

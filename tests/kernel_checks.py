@@ -61,16 +61,90 @@ def check_gemm_rowvec(M=256, N=320, K=64, seed=20):
     return _res(out, ref)
 
 
-def check_geglu(M=384, C=320, seed=30):
+def check_geglu(M=384, C=320, seed=30, out=None):
     A = _rand((M, C), seed).half()
     W = _rand((8 * C, C), seed + 1, 1 / math.sqrt(C)).half()
     b = _rand((8 * C,), seed + 2, 0.1).half()
     wp, bp = ops.pack_geglu(W, b)
-    out = ops.gemm(A, wp, bias=bp, mode=ops.EPI_GEGLU)
+    out = ops.gemm(A, wp, bias=bp, mode=ops.EPI_GEGLU, out=out)
     h = A.float() @ W.float().t() + b.float()
     v, g = h.chunk(2, -1)
     ref = v * F.gelu(g)
     return _res(out, ref)
+
+
+def _all(*rs):
+    """Merges sub-results: ok only if every one is."""
+    r = dict(max(rs, key=lambda x: x["err"] / max(x["tol"], 1e-30)))
+    r["ok"] = all(x["ok"] for x in rs)
+    return r
+
+
+def _flag(ok, what):
+    """A yes/no property as a result (err 1 when it fails)."""
+    return {"err": 0.0 if ok else 1.0, "ref": 0.0, "tol": 0.5, "ok": bool(ok), "what": what}
+
+
+def ln_sums_res(out, sums, bn, rel=1e-5):
+    """The (sum, sum of squares) slices a GEMM epilogue wrote, slice j = output columns [j bn, (j + 1) bn), against fp64
+    sums over the fp16 values it stored: relative to the sum of |x| (resp. of x^2) of the row."""
+    x = out.double()
+    M, N = x.shape
+    rs = []
+    for j in range(-(-N // bn)):
+        xs = x[:, j * bn:(j + 1) * bn]
+        got = sums[j].double()
+        err_s = ((got[:, 0] - xs.sum(1)).abs() / xs.abs().sum(1).clamp_min(1e-30)).max().item()
+        err_q = ((got[:, 1] - (xs * xs).sum(1)).abs() / (xs * xs).sum(1).clamp_min(1e-30)).max().item()
+        rs.append({"err": max(err_s, err_q), "ref": 1.0, "tol": rel, "ok": max(err_s, err_q) <= rel})
+    return _all(*rs)
+
+
+def check_gemm_residual_inplace(M, N, K, seed, ln_bn=None):
+    """out = fp16(fp16(A W^T + b) + R) written over R itself (the transformer's out1 / out2 / ff2 / proj_out calls:
+    residual is out).  ln_bn: also emit the LayerNorm row-statistics slices at that forced tile width (0 = automatic:
+    only the sum over the slices is checked, the slice width being unknown)."""
+    A = _rand((M, K), seed).half()
+    W = _rand((N, K), seed + 1, 1 / math.sqrt(K)).half()
+    b = _rand((N,), seed + 2).float()
+    R = (_rand((M, N), seed + 3) * 1.5 - 0.3).half()
+    ref = ((A.float() @ W.float().t() + b).half().float() + R.float()).half()
+    out = R.clone()
+    sums = None
+    if ln_bn is not None:
+        sums = torch.zeros((ops.max_column_tiles(N, ln_bn), M, 2), dtype=torch.float32, device=DEV)
+    ops.gemm(A, W, bias=b, residual=out, out=out, ln_sums=sums, force_bn=ln_bn or 0)
+    r = _res(out, ref)
+    if ln_bn is None:
+        return r
+    if ln_bn:
+        return _all(r, ln_sums_res(out, sums, ln_bn))
+    return _all(r, ln_sums_res(out, sums.sum(0, keepdim=True), N))     # one "slice" of all N columns
+
+
+def check_gemm_rows_untouched(M, N, K, bn=0, residual=False, ln_sums=False, geglu=False, seed=0, pad=70):
+    """`out` (and the row-statistics slices) are views into NaN-filled buffers: rows >= M of the output and slices past
+    the GEMM's column tiles must still be NaN afterwards."""
+    if geglu:
+        buf = torch.full((M + pad, 4 * K), float("nan"), dtype=torch.float16, device=DEV)
+        r = check_geglu(M=M, C=K, seed=seed, out=buf[:M])
+        return _all(r, _flag(torch.isnan(buf[M:]).all().item(), "rows >= M written"))
+    A = _rand((M, K), seed).half()
+    W = _rand((N, K), seed + 1, 1 / math.sqrt(K)).half()
+    b = _rand((N,), seed + 2).float()
+    R = _rand((M, N), seed + 3).half() if residual else None
+    buf = torch.full((M + pad, N), float("nan"), dtype=torch.float16, device=DEV)
+    nt = -(-N // bn)
+    sbuf = torch.full((nt + 2, M, 2), float("nan"), dtype=torch.float32, device=DEV) if ln_sums else None
+    out = ops.gemm(A, W, bias=b, residual=R, out=buf[:M], ln_sums=sbuf, force_bn=bn)
+    ref = A.float() @ W.float().t() + b
+    if residual:
+        ref = ref + R.float()
+    rs = [_res(out, ref), _flag(torch.isnan(buf[M:]).all().item(), "rows >= M written")]
+    if ln_sums:
+        rs.append(ln_sums_res(out, sbuf[:nt], bn))
+        rs.append(_flag(torch.isnan(sbuf[nt:]).all().item(), "slices >= n_tiles written"))
+    return _all(*rs)
 
 
 # ---------------------------------------------------------------------------------------------------- conv
@@ -120,6 +194,32 @@ def check_conv_out(n=2, H=16, W=16, ci=320, co=4, seed=60):
     return _conv_odd(n, H, W, ci, co, seed)
 
 
+def check_conv_rows_untouched(n, H, W, ci, co, seed, pad=70):
+    """The conv output is a view into a NaN-filled buffer: pixels past the problem (the padding of the conv tiles) must
+    not be stored anywhere."""
+    x = _rand((n, H, W, ci), seed).half()
+    w = _rand((co, ci, 3, 3), seed + 1, 1 / math.sqrt(9 * ci)).half()
+    b = _rand((co,), seed + 2).float()
+    M = n * H * W
+    buf = torch.full((M + pad, co), float("nan"), dtype=torch.float16, device=DEV)
+    out = ops.conv3x3(x, ops.pack_conv3x3(w), bias=b, out=buf[:M].view(n, H, W, co))
+    return _all(_res(out, _conv_ref(x, w, b)), _flag(torch.isnan(buf[M:]).all().item(), "pixels >= M written"))
+
+
+def check_conv_temb_table(B=2, Fr=3, H=16, W=16, ci=320, co=320, width=3200, off=640, seed=200):
+    """Resnet conv1 as the UNet runs it: the time-embedding add reads a column slice of ONE table shared by all resnets
+    (row stride = the table's width), one row per batch element = per F H W pixels (resnet.py: conv1 + time_emb_proj)."""
+    n = B * Fr
+    x = _rand((n, H, W, ci), seed).half()
+    w = _rand((co, ci, 3, 3), seed + 1, 1 / math.sqrt(9 * ci)).half()
+    b = _rand((co,), seed + 2).float()
+    table = _rand((B, width), seed + 3).float()
+    rv = table[:, off:off + co]
+    out = ops.conv3x3(x, ops.pack_conv3x3(w), bias=b, rowvec=rv, imgs_per_batch=Fr)
+    ref = _conv_ref(x, w, b) + rv.repeat_interleave(Fr, 0)[:, None, None, :]
+    return _res(out, ref)
+
+
 def check_conv_s2(n=2, H=16, W=16, ci=320, co=320, seed=70):
     x = _rand((n, H, W, ci), seed).half()
     w = _rand((co, ci, 3, 3), seed + 1, 1 / math.sqrt(9 * ci)).half()
@@ -139,11 +239,12 @@ def check_upsample_conv(n=2, H=8, W=8, ci=640, co=640, seed=75):
     return _res(out, ref)
 
 
-def check_conv_in(n=4, H=16, W=16, seed=80):
+def check_conv_in(n=4, H=16, W=16, seed=80, tc=False):
+    """tc=False: the direct CUDA-core kernel; tc=True: patch rows + tensor-core GEMM (K = 64), the UNet's path."""
     x = _rand((n, H, W, 4), seed).half()
     w = _rand((320, 4, 3, 3), seed + 1, 1 / 6).half()
     b = _rand((320,), seed + 2).float()
-    out = ops.conv_in(x, w, b)
+    out = ops.conv_in(x, w, b) if tc else ops.conv_in(x, w, b, scratch=None)
     return _res(out, _conv_ref(x, w, b))
 
 
@@ -173,6 +274,32 @@ def check_groupnorm(B=2, Fr=3, H=8, W=8, c1=320, c2=0, per_frame=False, silu=Tru
     if silu:
         ref = F.silu(ref)
     return _res(out, ref.permute(0, 2, 3, 1))
+
+
+def check_groupnorm_frame_shards(k, B=2, Fr=16, H=64, W=64, c1=320, c2=0, eps=1e-5, seed=180, mean=3.0):
+    """The frame-sharded 5-D GroupNorm of the resnets on one GPU: the frames of [B F, H, W, C] are split into k shards,
+    every shard ADDS its statistics into one zeroed buffer (zero_first = False: what the all-reduce of the per-rank sums
+    produces), and every shard is normalised with count_scale = k.  The concatenation must equal the unsharded norm."""
+    n, fs = B * Fr, Fr // k
+    x1 = (_rand((n, H, W, c1), seed) * 1.5 + mean).half()
+    x2 = (_rand((n, H, W, c2), seed + 1) * 0.7 - 0.2).half() if c2 else None
+    C = c1 + c2
+    gamma = (1 + 0.1 * _rand((C,), seed + 2)).float()
+    beta = (0.1 * _rand((C,), seed + 3)).float()
+
+    def shard(t, s):
+        return None if t is None else t.view(B, Fr, H, W, -1)[:, s * fs:(s + 1) * fs].reshape(B * fs, H, W, -1).contiguous()
+
+    sums = torch.zeros((B, 32, 2), dtype=torch.float32, device=DEV)
+    for s in range(k):
+        ops.groupnorm_stats(shard(x1, s), sums, 32, fs, x2=shard(x2, s), zero_first=False)
+    outs = [ops.groupnorm_apply(shard(x1, s), sums, gamma, beta, 32, eps, fs, count_scale=k, silu=True, x2=shard(x2, s))
+            for s in range(k)]
+    out = torch.cat([o.view(B, fs, H, W, C) for o in outs], 1).reshape(n, H, W, C)
+    x = x1 if x2 is None else torch.cat([x1, x2], -1)
+    x5 = x.float().view(B, Fr, H, W, C).permute(0, 4, 1, 2, 3)                 # [B, C, F, H, W]
+    ref = F.silu(F.group_norm(x5, 32, gamma, beta, eps)).permute(0, 2, 3, 4, 1).reshape(n, H, W, C)
+    return _res(out, ref)
 
 
 def check_layernorm(rows=1000, C=320, pe=False, seed=110):
@@ -250,6 +377,29 @@ def check_linear_ln_linear(rows=2000, K0=320, C=320, N=960, residual=False, gegl
     return r2
 
 
+def check_ln_fuse_pe_motion(B=2, Ft=16, hw=64, C=320, seed=170, mean=10.0):
+    """The motion module's chain (motion_module.py: proj_in / attention output -> norm + positional encoding -> to_qkv):
+    the producer GEMM (+ residual) writes the row statistics, the consumer folds the LayerNorm from those slices and adds
+    the temporal PE as a row vector, rows ordered [(b f), hw] -> PE row (row // hw) % Ft.  The rows' mean is about 8x
+    their spread: the slices give the variance as E[x^2] - mean^2."""
+    M = B * Ft * hw
+    x0 = _rand((M, C), seed).half()
+    W0 = _rand((C, C), seed + 1, 1 / math.sqrt(C)).half()
+    b0 = (_rand((C,), seed + 2) * 0.1 + mean).float()
+    R = (_rand((M, C), seed + 3) * 0.5).half()
+    gamma = (1 + 0.1 * _rand((C,), seed + 4)).float()
+    beta = (0.1 * _rand((C,), seed + 5)).float()
+    table = _rand((24, C), seed + 6).float()
+    W = _rand((3 * C, C), seed + 7, 1 / math.sqrt(C)).half()
+    x, out = ops.linear_ln_linear(x0, W0, b0, W, gamma, beta, residual=R, pe=table, hw=hw, frames=Ft)
+    xr = (x0.float() @ W0.float().t() + b0).half().float() + R.float()
+    xf = x.float()
+    spread = xf.std(1).mean().item()
+    dominant = _flag(xf.mean(1).abs().min().item() >= 8 * spread, "row mean >= 8x spread")
+    y = F.layer_norm(xf, (C,), gamma, beta, 1e-5) + table[(torch.arange(M, device=DEV) // hw) % Ft]
+    return _all(_res(out, y @ W.float().t()), _res(x, xr), dominant)
+
+
 # ---------------------------------------------------------------------------------------------------- attention
 def _mha_ref(q, k, v, heads):
     B, nq, C = q.shape
@@ -292,7 +442,41 @@ def check_temporal_attention(B=2, Fr=16, HW=20, C=320, seed=140):
     t = qkv.permute(0, 2, 1, 3).reshape(B * HW, Fr, 3 * C)
     ref = _mha_ref(t[..., :C], t[..., C:2 * C], t[..., 2 * C:], 8)
     ref = ref.reshape(B, HW, Fr, C).permute(0, 2, 1, 3)
-    return _res(out, ref)
+    r = _res(out, ref)
+    if Fr == 1:                  # one frame: softmax over one key = 1, the output is v to fp16 rounding
+        v = qkv[..., 2 * C:].float()
+        r = _all(r, _flag(((out.float() - v).abs() <= v.abs() * 2 ** -11).all().item(), "F = 1 output != v"))
+    return r
+
+
+def check_attn_dominant_key(B=2, Fr=1, N=300, C=320, nk=None, heads=8, where="first", seed=190, min_rows=0.75):
+    """One key takes >= 90 % of the softmax mass for most rows (the BOS-token pattern of SD cross-attention maps): every
+    query's first head coordinate is a, the dominant key's is b (its other coordinates 0), so its logit is a b / sqrt(d)
+    ~ 14 against N(0, ~1.2) for the rest.  where = "first": cross-attention, key 0; "last": self-attention, key N - 1
+    (with N = 64 k + 1, alone in the last key tile: the row maximum jumps on the final tile)."""
+    d = C // heads
+    a, b = 4.0, 14.0 * math.sqrt(d) / 4.0
+    cross = nk is not None
+    q = _rand((B * Fr, N, C), seed).half() if cross else None
+    if cross:
+        kv = _rand((B, nk, 2 * C), seed + 1).half()
+        k, v = kv[..., :C], kv[..., C:]
+    else:
+        qkv = _rand((B, N, 3 * C), seed).half()
+        q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
+    j = 0 if where == "first" else k.shape[1] - 1
+    for h in range(heads):
+        q[..., h * d] = a
+        k[:, j, h * d:(h + 1) * d] = 0
+        k[:, j, h * d] = b
+    kr = k.repeat_interleave(Fr, 0) if cross else k
+    vr = v.repeat_interleave(Fr, 0) if cross else v
+    qh = q.float().reshape(q.shape[0], N, heads, d).transpose(1, 2)
+    kh = kr.float().reshape(kr.shape[0], -1, heads, d).transpose(1, 2)
+    mass = (qh @ kh.transpose(-1, -2) * d ** -0.5).softmax(-1)[..., j]
+    dominant = _flag((mass >= 0.9).float().mean().item() >= min_rows, "dominant key holds >= 90 % for too few rows")
+    out = ops.attention(q, k, v, heads, kv_div=Fr) if cross else ops.attention(q, k, v, heads)
+    return _all(_res(out, _mha_ref(q, kr, vr, heads)), dominant)
 
 
 # ---------------------------------------------------------------------------------------------------- step
@@ -305,6 +489,36 @@ def check_cfg_ddim(dtype=torch.float16, seed=150):
     x0 = (x.float() - math.sqrt(1 - a_t) * e) / math.sqrt(a_t)
     ref = math.sqrt(a_p) * x0 + math.sqrt(1 - a_p) * e
     return _res(out, ref, rel=2 ** -9, abs_=1e-3)
+
+
+def check_cfg_ddim_nocfg(dtype=torch.float16, seed=151):
+    """cfg = 0 (the inversion loop): eps2 is ONE prediction [1, n], no guidance combine."""
+    eps = _rand((1, 4, 4, 8, 8), seed).to(dtype)
+    x = _rand((1, 4, 4, 8, 8), seed + 1).to(dtype)
+    a_t, a_p = 0.0058, 0.0047
+    out = ops.cfg_ddim_step(eps, x, 7.5, a_t, a_p, cfg=False)
+    e = eps.float()
+    ref = math.sqrt(a_p) * (x.float() - math.sqrt(1 - a_t) * e) / math.sqrt(a_t) + math.sqrt(1 - a_p) * e
+    return _res(out, ref, rel=2 ** -9, abs_=1e-3)
+
+
+def check_cfg_ddim_devcoef(dtype=torch.float16, seed=152):
+    """Coefficients (c_x, c_e) from device memory (the graph-replayed step): against the host formula, and bit-identical
+    to the host-alpha launch when they are computed in float32 by the library's own expression."""
+    import numpy as np
+    eps2 = _rand((2, 4, 4, 8, 8), seed).to(dtype)
+    x = _rand((1, 4, 4, 8, 8), seed + 1).to(dtype)
+    a_t, a_p, g = 0.0047, 0.0058, 7.5
+    at, ap = np.float32(a_t), np.float32(a_p)
+    one = np.float32(1.0)
+    c_x = np.sqrt(ap) / np.sqrt(at)
+    c_e = np.sqrt(one - ap) - np.sqrt(ap) * np.sqrt(one - at) / np.sqrt(at)
+    coef = torch.tensor([c_x, c_e], dtype=torch.float32, device=DEV)
+    out = ops.cfg_ddim_step(eps2, x, g, coef=coef)
+    host = ops.cfg_ddim_step(eps2, x, g, a_t, a_p)
+    e = eps2[0:1].float() + g * (eps2[1:2].float() - eps2[0:1].float())
+    ref = math.sqrt(a_p) * (x.float() - math.sqrt(1 - a_t) * e) / math.sqrt(a_t) + math.sqrt(1 - a_p) * e
+    return _all(_res(out, ref, rel=2 ** -9, abs_=1e-3), _flag(torch.equal(out, host), "device coefficients != host alphas"))
 
 
 def with_option(name, value, fn, restore):
@@ -477,4 +691,59 @@ CHECKS = {
     "temporal_attn_f24": lambda: check_temporal_attention(B=1, Fr=24, HW=5, C=640),
     "cfg_ddim_f16": lambda: check_cfg_ddim(torch.float16),
     "cfg_ddim_f32": lambda: check_cfg_ddim(torch.float32),
+    # ---- the argument combinations the UNet forward passes to the GEMM
+    # resnet conv1: time-embedding row vector = a column slice of the table shared by all resnets, one row per F H W pixels
+    "conv_temb_table_320": lambda: check_conv_temb_table(),
+    "conv_temb_table_1280": lambda: check_conv_temb_table(H=8, W=8, ci=1280, co=1280, width=5120, off=2560, seed=201),
+    # residual is out (attention output projections, ff2, proj_out), with and without the LayerNorm row statistics
+    "gemm_residual_inplace_l0": lambda: check_gemm_residual_inplace(128 * 150 + 9, 320, 320, seed=210),
+    "gemm_residual_inplace_1280": lambda: check_gemm_residual_inplace(8192, 1280, 1280, seed=211),
+    "gemm_residual_inplace_lnsums_bn128": lambda: check_gemm_residual_inplace(128 * 40 + 9, 640, 320, seed=212, ln_bn=128),
+    "gemm_residual_inplace_lnsums_bn160": lambda: check_gemm_residual_inplace(128 * 40 + 9, 640, 320, seed=213, ln_bn=160),
+    "gemm_residual_inplace_lnsums_bn256": lambda: check_gemm_residual_inplace(128 * 40 + 9, 640, 320, seed=214, ln_bn=256),
+    "gemm_residual_inplace_lnsums_auto": lambda: check_gemm_residual_inplace(4096 + 37, 1280, 1280, seed=215, ln_bn=0),
+    # motion module: producer row statistics -> LayerNorm fold + temporal PE row vector (rv_mod = frames)
+    "ln_fuse_pe_motion_c320_hw64_f16": lambda: check_ln_fuse_pe_motion(B=2, Ft=16, hw=64, C=320, seed=170),
+    "ln_fuse_pe_motion_c1280_hw20_f24": lambda: check_ln_fuse_pe_motion(B=1, Ft=24, hw=20, C=1280, seed=171),
+    "ln_fuse_pe_motion_c1280_hw64_f16": lambda: check_ln_fuse_pe_motion(B=1, Ft=16, hw=64, C=1280, seed=172),
+    "ln_fuse_pe_motion_c320_hw20_f24": lambda: check_ln_fuse_pe_motion(B=2, Ft=24, hw=20, C=320, seed=173),
+    # nothing is written past row M of the output or past the used row-statistics slices
+    "gemm_rows_untouched_bn64": lambda: check_gemm_rows_untouched(128 * 5 + 9, 320, 320, bn=64, residual=True, ln_sums=True, seed=220),
+    "gemm_rows_untouched_bn128": lambda: check_gemm_rows_untouched(128 * 5 + 9, 640, 256, bn=128, ln_sums=True, seed=221),
+    "gemm_rows_untouched_bn160": lambda: check_gemm_rows_untouched(1000, 320, 320, bn=160, residual=True, seed=222),
+    "gemm_rows_untouched_bn256": lambda: check_gemm_rows_untouched(700, 768, 320, bn=256, residual=True, ln_sums=True, seed=223),
+    "gemm_rows_untouched_geglu": lambda: check_gemm_rows_untouched(1000, 0, 320, geglu=True, seed=224),
+    "gemm_rows_untouched_conv_odd": lambda: check_conv_rows_untouched(3, 7, 12, 320, 320, seed=225),
+    "gemm_rows_untouched_conv_out": lambda: check_conv_rows_untouched(3, 7, 12, 320, 4, seed=226),
+    # ---- product paths without a kernel check before
+    "conv_in_tc_l0": lambda: check_conv_in(n=32, H=64, W=64, seed=81, tc=True),
+    "conv_in_tc_56x96": lambda: check_conv_in(n=4, H=56, W=96, seed=82, tc=True),
+    "cross_attn_d160_l2": lambda: check_cross_attention(B=2, Fr=16, N=256, C=1280, nk=77, seed=230),
+    "cross_attn_d160_mid": lambda: check_cross_attention(B=2, Fr=16, N=64, C=1280, nk=77, seed=231),
+    "cross_attn_d160_n336": lambda: check_cross_attention(B=2, Fr=4, N=336, C=1280, nk=77, seed=232),
+    "self_attn_d160_n256": lambda: check_self_attention(B=4, N=256, C=1280, seed=233),
+    "self_attn_d160_n336": lambda: check_self_attention(B=4, N=336, C=1280, seed=234),
+    # one key with >= 90 % of the softmax mass: first (cross, 77 keys) or alone in the last key tile (self, N = 64 k + 1)
+    "attn_dominant_key_cross_first_d40": lambda: check_attn_dominant_key(B=2, Fr=2, N=300, C=320, nk=77, seed=190),
+    "attn_dominant_key_cross_first_d80": lambda: check_attn_dominant_key(B=2, Fr=2, N=256, C=640, nk=77, seed=191),
+    "attn_dominant_key_cross_first_d160": lambda: check_attn_dominant_key(B=2, Fr=4, N=256, C=1280, nk=77, seed=192),
+    "attn_dominant_key_self_last_d40": lambda: check_attn_dominant_key(B=2, N=64 * 16 + 1, C=320, where="last", seed=193),
+    "attn_dominant_key_self_last_d80": lambda: check_attn_dominant_key(B=2, N=64 * 5 + 1, C=640, where="last", seed=194),
+    "attn_dominant_key_self_last_d160": lambda: check_attn_dominant_key(B=2, N=64 * 4 + 1, C=1280, where="last", seed=195),
+    "attn_dominant_key_self_last_d40_mma": with_option("attn_tc", 0, lambda: check_attn_dominant_key(
+        B=2, N=64 * 16 + 1, C=320, where="last", seed=193), 1),
+    "attn_dominant_key_cross_first_d40_mma": with_option("attn_tc", 0, lambda: check_attn_dominant_key(
+        B=2, Fr=2, N=300, C=320, nk=77, seed=190), 1),
+    "temporal_attn_f1_d40": lambda: check_temporal_attention(B=2, Fr=1, HW=64, C=320, seed=142),
+    "temporal_attn_f1_d160": lambda: check_temporal_attention(B=2, Fr=1, HW=20, C=1280, seed=143),
+    "temporal_attn_f2_d40": lambda: check_temporal_attention(B=2, Fr=2, HW=64, C=320, seed=144),
+    "temporal_attn_f2_d160": lambda: check_temporal_attention(B=2, Fr=2, HW=20, C=1280, seed=145),
+    # frame-sharded 5-D GroupNorm (statistics added into one buffer, count_scale = k) vs the unsharded norm
+    "gn5d_frame_shards_k2": lambda: check_groupnorm_frame_shards(2),
+    "gn5d_frame_shards_k4": lambda: check_groupnorm_frame_shards(4, seed=181),
+    "gn5d_frame_shards_k2_concat": lambda: check_groupnorm_frame_shards(2, B=1, H=32, W=32, c1=640, c2=320, mean=-2.0, seed=182),
+    "cfg_ddim_nocfg_f16": lambda: check_cfg_ddim_nocfg(torch.float16),
+    "cfg_ddim_nocfg_f32": lambda: check_cfg_ddim_nocfg(torch.float32),
+    "cfg_ddim_devcoef_f16": lambda: check_cfg_ddim_devcoef(torch.float16),
+    "cfg_ddim_devcoef_f32": lambda: check_cfg_ddim_devcoef(torch.float32),
 }

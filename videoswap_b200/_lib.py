@@ -34,6 +34,28 @@ _F = C.c_float
 _LL = C.c_longlong
 _SZ = C.c_size_t
 
+
+class GemmDescStruct(C.Structure):
+    """vs_gemm_desc: one launch of the tensor-core GEMM / implicit-GEMM convolution (see the header)."""
+    _fields_ = [
+        ("A", _P), ("K1", _I), ("lda1", _I),
+        ("A2", _P), ("K2", _I), ("lda2", _I),
+        ("Bw", _P),
+        ("M", _I), ("N", _I),
+        ("taps", _I),
+        ("sub_py", _I), ("sub_px", _I),
+        ("nimg", _I), ("H", _I), ("W", _I),
+        ("bias", _P),
+        ("rowvec", _P), ("ldrv", _I), ("pix_per_batch", _I), ("rv_mod", _I),
+        ("ln_stats", _P), ("ln_u", _P),
+        ("ln_parts", _P), ("ln_nparts", _I),
+        ("ln_sums_out", _P),
+        ("residual", _P), ("ldr", _I),
+        ("out", _P), ("ldc", _I),
+        ("mode", _I),
+        ("force_bn", _I),
+    ]
+
 _SIGNATURES = {
     "vs_last_error": (C.c_char_p, []),
     "vs_version": (_I, []),
@@ -66,11 +88,12 @@ _SIGNATURES = {
     "vs_cfg_ddim_step": (_I, [_P, _P, _P, _I, _SZ, _I, _F, _F, _F, _P]),
     "vs_cfg_ddim_step_dev": (_I, [_P, _P, _P, _I, _SZ, _I, _F, _P, _P]),
     "vs_adapter_level": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _F, _I, _F, _P, _P]),
-    "vs_gemm": (_I, [_P, _P, _I, _P, _I, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I]),
-    "vs_conv3x3": (_I, [_P, _P, _I, _P, _I, _P, _I, _I, _I, _I, _P, _P, _I, _P, _P]),
+    "vs_gemm_ex": (_I, [_P, C.POINTER(GemmDescStruct)]),
     "vs_pack_conv3x3": (_I, [_P, _P, _I, _I, _P]),
     "vs_pack_geglu": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "vs_groupnorm": (_I, [_P, _P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _P, _I, _P, _P]),
+    "vs_groupnorm_stats": (_I, [_P, _P, _I, _P, _I, _I, _I, _I, _I, _P, _I]),
+    "vs_groupnorm_apply": (_I, [_P, _P, _I, _P, _I, _I, _I, _I, _I, _P, _F, _P, _P, _I, _I, _P]),
     "vs_layernorm": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _I, _P]),
     "vs_ln_linear": (_I, [_P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "vs_unet_set_attention_hook": (_I, [_P, _P, _P, _I]),      # hook: CFUNCTYPE object or None
@@ -78,10 +101,11 @@ _SIGNATURES = {
     "vs_attention_apply_probs": (_I, [_P, _P, _P, _I, _P, _I, _I, _I, _I, _I, _I, _LL, _LL, _I]),
     "vs_blend_mask": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _I, _I, _F, _I, _P]),
     "vs_latent_blend": (_I, [_P, _P, _P, _P, _I, _I, _I, _I]),
-    "vs_linear_ln_linear": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _I, _P]),
+    "vs_linear_ln_linear": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _P, _I, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P,
+                                 _P, _I, _P]),
     "vs_attention": (_I, [_P, _P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _LL, _LL, _LL, _I]),
     "vs_temporal_attention": (_I, [_P, _P, _P, _I, _I, _I, _I, _I]),
-    "vs_conv_in": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _I, _P]),
+    "vs_conv_in": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _I, _P, _P]),
     "vs_upsample2x": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "vs_upsample_conv3x3": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P, _P]),
     "vs_conv3x3_s2": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P, _P]),

@@ -38,25 +38,25 @@ extern "C" int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0
   return adapter_splat(st, feat, d_tracks, d_mask, F, P, C, h, w, rate, coord_fp16, scale, (__half*)d_map);
 }
 
-extern "C" int vs_gemm(void* stream, const void* d_A, int K1, const void* d_A2, int K2, const void* d_W, int M, int N,
-                       const float* d_bias, const float* d_rowvec, int pix_per_batch, const void* d_residual, void* d_out,
-                       int mode, int force_bn) {
+extern "C" int vs_gemm_ex(void* stream, const vs_gemm_desc* d) {
+  VS_REQUIRE(d != nullptr, "vs_gemm_ex: null descriptor");
   GemmArgs g;
-  g.A = (const __half*)d_A; g.K1 = K1; g.lda1 = K1; g.A2 = (const __half*)d_A2; g.K2 = K2; g.lda2 = K2;
-  g.Bw = (const __half*)d_W; g.M = M; g.N = N; g.bias = d_bias; g.rowvec = d_rowvec; g.pix_per_batch = pix_per_batch;
-  g.residual = (const __half*)d_residual; g.ldr = (mode == EPI_GEGLU) ? N / 2 : N;
-  g.out = (__half*)d_out; g.ldc = (mode == EPI_GEGLU) ? N / 2 : N; g.mode = mode; g.force_bn = force_bn;
-  return gemm_tc((cudaStream_t)stream, g);
-}
-
-extern "C" int vs_conv3x3(void* stream, const void* d_x, int C1, const void* d_x2, int C2, const void* d_w, int nimg, int H,
-                          int W, int Cout, const float* d_bias, const float* d_rowvec, int imgs_per_batch,
-                          const void* d_residual, void* d_out) {
-  GemmArgs g;
-  g.A = (const __half*)d_x; g.K1 = C1; g.lda1 = C1; g.A2 = (const __half*)d_x2; g.K2 = C2; g.lda2 = C2;
-  g.Bw = (const __half*)d_w; g.taps = 9; g.nimg = nimg; g.H = H; g.W = W; g.M = nimg * H * W; g.N = Cout; g.bias = d_bias;
-  g.rowvec = d_rowvec; g.pix_per_batch = imgs_per_batch * H * W; g.residual = (const __half*)d_residual; g.ldr = Cout;
-  g.out = (__half*)d_out; g.ldc = Cout;
+  g.A = (const __half*)d->A; g.K1 = d->K1; g.lda1 = d->lda1;
+  g.A2 = (const __half*)d->A2; g.K2 = d->K2; g.lda2 = d->lda2;
+  g.Bw = (const __half*)d->Bw;
+  g.M = d->M; g.N = d->N;
+  g.taps = d->taps;
+  g.sub_py = d->sub_py; g.sub_px = d->sub_px;
+  g.nimg = d->nimg; g.H = d->H; g.W = d->W;
+  g.bias = d->bias;
+  g.rowvec = d->rowvec; g.ldrv = d->ldrv; g.pix_per_batch = d->pix_per_batch; g.rv_mod = d->rv_mod;
+  g.ln_stats = d->ln_stats; g.ln_u = d->ln_u;
+  g.ln_parts = d->ln_parts; g.ln_nparts = d->ln_nparts;
+  g.ln_sums_out = d->ln_sums_out;
+  g.residual = (const __half*)d->residual; g.ldr = d->ldr;
+  g.out = (__half*)d->out; g.ldc = d->ldc;
+  g.mode = d->mode;
+  g.force_bn = d->force_bn;
   return gemm_tc((cudaStream_t)stream, g);
 }
 
@@ -80,6 +80,20 @@ extern "C" int vs_groupnorm(void* stream, const void* d_x1, int c1, const void* 
   if (int e = groupnorm_stats(st, (const __half*)d_x1, c1, (const __half*)d_x2, c2, nimg, hw, imgs_per_set, groups, d_sums)) return e;
   return groupnorm_apply(st, (const __half*)d_x1, c1, (const __half*)d_x2, c2, nimg, hw, imgs_per_set, groups, d_sums, eps,
                          d_gamma, d_beta, silu != 0, (__half*)d_out);
+}
+extern "C" int vs_groupnorm_stats(void* stream, const void* d_x1, int c1, const void* d_x2, int c2, int nimg, int hw,
+                                  int imgs_per_set, int groups, float* d_sums, int zero_first) {
+  VS_REQUIRE(d_sums != nullptr, "vs_groupnorm_stats: null sums");
+  return groupnorm_stats((cudaStream_t)stream, (const __half*)d_x1, c1, (const __half*)d_x2, c2, nimg, hw, imgs_per_set, groups,
+                         d_sums, zero_first != 0);
+}
+extern "C" int vs_groupnorm_apply(void* stream, const void* d_x1, int c1, const void* d_x2, int c2, int nimg, int hw,
+                                  int imgs_per_set, int groups, const float* d_sums, float eps, const float* d_gamma,
+                                  const float* d_beta, int silu, int count_scale, void* d_out) {
+  VS_REQUIRE(d_sums && d_out, "vs_groupnorm_apply: null pointer");
+  VS_REQUIRE(count_scale >= 1, "vs_groupnorm_apply: count_scale must be >= 1");
+  return groupnorm_apply((cudaStream_t)stream, (const __half*)d_x1, c1, (const __half*)d_x2, c2, nimg, hw, imgs_per_set, groups,
+                         d_sums, eps, d_gamma, d_beta, silu != 0, (__half*)d_out, count_scale);
 }
 extern "C" int vs_layernorm(void* stream, const void* d_x, int rows, int C, const float* d_gamma, const float* d_beta,
                             const float* d_pe, int hw, int F, void* d_out) {
@@ -133,10 +147,11 @@ extern "C" int vs_latent_blend(void* stream, const void* d_x_src, void* d_x_tgt,
 }
 extern "C" int vs_linear_ln_linear(void* stream, const void* d_x0, int M, int K0, const void* d_w0, const float* d_b0,
                                    const void* d_residual, int C, void* d_x, const void* d_w, const float* d_bias, int N,
-                                   const float* d_gamma, const float* d_beta, int mode, void* d_wf, float* d_u, float* d_c,
-                                   float* d_parts, int parts_capacity, void* d_out) {
+                                   const float* d_gamma, const float* d_beta, const float* d_pe, int pe_len, int hw,
+                                   int frames, int mode, void* d_wf, float* d_u, float* d_c, float* d_cpe, float* d_parts,
+                                   int parts_capacity, void* d_out) {
   cudaStream_t st = (cudaStream_t)stream;
-  if (int e = ln_fold(st, (const __half*)d_w, N, C, d_gamma, d_beta, d_bias, nullptr, 0, (__half*)d_wf, d_u, d_c, nullptr)) return e;
+  if (int e = ln_fold(st, (const __half*)d_w, N, C, d_gamma, d_beta, d_bias, d_pe, pe_len, (__half*)d_wf, d_u, d_c, d_cpe)) return e;
   GemmArgs g0;                                  // producer: x = x0 W0^T + b0 (+ residual), row statistics from its epilogue
   g0.A = (const __half*)d_x0; g0.K1 = K0; g0.lda1 = K0; g0.Bw = (const __half*)d_w0; g0.M = M; g0.N = C; g0.bias = d_b0;
   g0.residual = (const __half*)d_residual; g0.ldr = C; g0.out = (__half*)d_x; g0.ldc = C; g0.ln_sums_out = d_parts;
@@ -146,6 +161,7 @@ extern "C" int vs_linear_ln_linear(void* stream, const void* d_x0, int M, int K0
   GemmArgs g;                                   // consumer: LayerNorm(x) folded into this GEMM, statistics from the slices
   g.A = (const __half*)d_x; g.K1 = C; g.lda1 = C; g.Bw = (const __half*)d_wf; g.M = M; g.N = N; g.bias = d_c;
   g.ln_parts = d_parts; g.ln_nparts = parts; g.ln_u = d_u; g.out = (__half*)d_out; g.ldc = mode == EPI_GEGLU ? N / 2 : N; g.mode = mode;
+  if (d_pe) { g.rowvec = d_cpe; g.ldrv = N; g.pix_per_batch = hw; g.rv_mod = frames; }
   return gemm_tc(st, g);
 }
 extern "C" int vs_attention(void* stream, const void* d_q, int ldq, const void* d_k, int ldk, const void* d_v, int ldv,
@@ -158,8 +174,9 @@ extern "C" int vs_temporal_attention(void* stream, const void* d_qkv, void* d_o,
   return temporal_attention((cudaStream_t)stream, (const __half*)d_qkv, (__half*)d_o, B, F, HW, C, heads);
 }
 extern "C" int vs_conv_in(void* stream, const void* d_x, int nimg, int H, int W, int cin, const void* d_w, const float* d_bias,
-                          int cout, void* d_out) {
-  return conv_in_3x3((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, cin, (const __half*)d_w, d_bias, cout, (__half*)d_out);
+                          int cout, void* d_scratch, void* d_out) {
+  return conv_in_3x3((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, cin, (const __half*)d_w, d_bias, cout, (__half*)d_out,
+                     (__half*)d_scratch);
 }
 extern "C" int vs_upsample2x(void* stream, const void* d_x, int nimg, int H, int W, int C, void* d_out) {
   return upsample_nearest2x((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, C, (__half*)d_out);

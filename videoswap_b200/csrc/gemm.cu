@@ -420,8 +420,10 @@ int launch(cudaStream_t st, const GemmParams& p) {
     configured = true;
   }
   const int total = ((p.m_tiles + 1) / 2) * p.n_tiles;   // units of two tiles
-  return launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(total < num_sms() ? total : num_sms()), dim3(GEMM_THREADS), C::SMEM_BYTES,
-                    st, 1, p);
+  int ctas = num_sms();
+  const int cap = get_option("gemm_ctas");              // > 0: fewer CTAs, each walking more units (another tile schedule)
+  if (cap > 0 && cap < ctas) ctas = cap;
+  return launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(total < ctas ? total : ctas), dim3(GEMM_THREADS), C::SMEM_BYTES, st, 1, p);
 }
 
 template <int BN>

@@ -38,17 +38,63 @@ def _chk32(*ts):
             assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), "expected contiguous fp32 CUDA tensor"
 
 
-def gemm(A, W, bias=None, residual=None, A2=None, rowvec=None, pix_per_batch=1, mode=EPI_LINEAR, force_bn=0):
-    """out[M, N] = [A | A2] @ W^T (+bias +rowvec[row // pix_per_batch] +residual); GEGLU mode expects packed W/bias."""
+def _ptr(t: Optional[torch.Tensor]) -> int:
+    return 0 if t is None else t.data_ptr()
+
+
+def _out16(out, shape, device):
+    """The caller's output tensor (checked) or a new one."""
+    if out is None:
+        return torch.empty(shape, dtype=torch.float16, device=device)
+    _chk16(out)
+    assert tuple(out.shape) == tuple(shape), f"out has shape {tuple(out.shape)}, expected {tuple(shape)}"
+    return out
+
+
+def _chk_rowvec(rv, N):
+    """fp32 [rows, N] with unit column stride: a whole table or a column slice of a wider one (row stride = ldrv)."""
+    if rv is not None:
+        assert rv.is_cuda and rv.dtype == torch.float32 and rv.dim() == 2 and rv.shape[1] == N and rv.stride(1) == 1, \
+            "expected an fp32 [rows, N] CUDA row-vector table with unit column stride"
+
+
+def max_column_tiles(N, force_bn=0):
+    """Upper bound on the column tiles of a GEMM (= LayerNorm partial-sum slices it writes): the automatic tile width is
+    64 for N <= 64 and at least 128 otherwise."""
+    bn = force_bn or (64 if N <= 64 else 128)
+    return -(-N // bn)
+
+
+def _gemm_ex(**fields):
+    d = _lib.GemmDescStruct()
+    d.taps = 1
+    d.pix_per_batch = 1
+    for k, v in fields.items():
+        setattr(d, k, v)
+    _lib.call("vs_gemm_ex", _stream(), C.byref(d))
+
+
+def gemm(A, W, bias=None, residual=None, A2=None, rowvec=None, pix_per_batch=1, mode=EPI_LINEAR, force_bn=0, out=None,
+         ln_sums=None):
+    """out[M, N] = [A | A2] @ W^T (+bias +rowvec[row // pix_per_batch] +residual); GEGLU mode expects packed W/bias.
+    out: the caller's [M, N] ([M, N/2] for GEGLU) tensor; it may be `residual` itself (in-place residual add, as the UNet's
+    attention output projections run).  rowvec may be a column slice of a wider table.  ln_sums: [slices, M, 2] fp32
+    (slices >= max_column_tiles(N, force_bn)) that receives, per column tile, each row's (sum, sum of squares) of the
+    stored fp16 outputs."""
     _chk16(A, W, residual, A2)
-    _chk32(bias, rowvec)
+    _chk32(bias, ln_sums)
     M, K1 = A.shape
     K2 = 0 if A2 is None else A2.shape[1]
     N = W.shape[0]
     assert W.shape[1] == K1 + K2
-    out = torch.empty((M, N // 2 if mode == EPI_GEGLU else N), dtype=torch.float16, device=A.device)
-    _lib.call("vs_gemm", _stream(), _p(A), K1, _p(A2), K2, _p(W), M, N, _p(bias), _p(rowvec), pix_per_batch,
-              _p(residual), _p(out), mode, force_bn)
+    _chk_rowvec(rowvec, N)
+    oc = N // 2 if mode == EPI_GEGLU else N
+    out = _out16(out, (M, oc), A.device)
+    if ln_sums is not None:
+        assert ln_sums.dim() == 3 and ln_sums.shape[1:] == (M, 2) and ln_sums.shape[0] >= max_column_tiles(N, force_bn)
+    _gemm_ex(A=_ptr(A), K1=K1, lda1=K1, A2=_ptr(A2), K2=K2, lda2=K2, Bw=_ptr(W), M=M, N=N, bias=_ptr(bias),
+             rowvec=_ptr(rowvec), ldrv=0 if rowvec is None else rowvec.stride(0), pix_per_batch=pix_per_batch,
+             ln_sums_out=_ptr(ln_sums), residual=_ptr(residual), ldr=oc, out=_ptr(out), ldc=oc, mode=mode, force_bn=force_bn)
     return out
 
 
@@ -71,16 +117,19 @@ def pack_geglu(w, b):
     return wout, bout
 
 
-def conv3x3(x, w_packed, bias=None, x2=None, rowvec=None, imgs_per_batch=1, residual=None):
-    """x: [N, H, W, C1] (+x2 [N, H, W, C2] channel concat), w_packed [Co, 9*(C1+C2)] -> [N, H, W, Co]."""
+def conv3x3(x, w_packed, bias=None, x2=None, rowvec=None, imgs_per_batch=1, residual=None, out=None):
+    """x: [N, H, W, C1] (+x2 [N, H, W, C2] channel concat), w_packed [Co, 9*(C1+C2)] -> [N, H, W, Co].
+    rowvec[image // imgs_per_batch] is added (may be a column slice of a wider table); out: the caller's output tensor."""
     _chk16(x, w_packed, x2, residual)
-    _chk32(bias, rowvec)
+    _chk32(bias)
     n, H, W, C1 = x.shape
     C2 = 0 if x2 is None else x2.shape[3]
     co = w_packed.shape[0]
-    out = torch.empty((n, H, W, co), dtype=torch.float16, device=x.device)
-    _lib.call("vs_conv3x3", _stream(), _p(x), C1, _p(x2), C2, _p(w_packed), n, H, W, co, _p(bias), _p(rowvec),
-              imgs_per_batch, _p(residual), _p(out))
+    _chk_rowvec(rowvec, co)
+    out = _out16(out, (n, H, W, co), x.device)
+    _gemm_ex(A=_ptr(x), K1=C1, lda1=C1, A2=_ptr(x2), K2=C2, lda2=C2, Bw=_ptr(w_packed), M=n * H * W, N=co, taps=9, nimg=n,
+             H=H, W=W, bias=_ptr(bias), rowvec=_ptr(rowvec), ldrv=0 if rowvec is None else rowvec.stride(0),
+             pix_per_batch=imgs_per_batch * H * W, residual=_ptr(residual), ldr=co, out=_ptr(out), ldc=co)
     return out
 
 
@@ -120,6 +169,31 @@ def groupnorm(x1, gamma, beta, groups, eps, imgs_per_set=1, silu=False, x2=None)
     return out
 
 
+def groupnorm_stats(x1, sums, groups, imgs_per_set, x2=None, zero_first=True):
+    """Adds each set's per-group (sum, sum of squares) of x1 (+ x2) into sums [n / imgs_per_set, groups, 2] fp32 (zeroed
+    first only with zero_first): the statistics half of the GroupNorm, as a frame shard computes it."""
+    _chk16(x1, x2)
+    _chk32(sums)
+    n, H, W, c1 = x1.shape
+    c2 = 0 if x2 is None else x2.shape[3]
+    assert tuple(sums.shape) == (n // imgs_per_set, groups, 2)
+    _lib.call("vs_groupnorm_stats", _stream(), _p(x1), c1, _p(x2), c2, n, H * W, imgs_per_set, groups, _p(sums),
+              int(zero_first))
+    return sums
+
+
+def groupnorm_apply(x1, sums, gamma, beta, groups, eps, imgs_per_set, count_scale=1, silu=False, x2=None):
+    """Normalises x1 (+ x2) with `sums` that cover count_scale times the local elements (all-reduced frame shards)."""
+    _chk16(x1, x2)
+    _chk32(sums, gamma, beta)
+    n, H, W, c1 = x1.shape
+    c2 = 0 if x2 is None else x2.shape[3]
+    out = torch.empty((n, H, W, c1 + c2), dtype=torch.float16, device=x1.device)
+    _lib.call("vs_groupnorm_apply", _stream(), _p(x1), c1, _p(x2), c2, n, H * W, imgs_per_set, groups, _p(sums), eps,
+              _p(gamma), _p(beta), int(silu), int(count_scale), _p(out))
+    return out
+
+
 def layernorm(x, gamma, beta, pe=None, hw=1, F=1):
     _chk16(x)
     _chk32(gamma, beta, pe)
@@ -147,11 +221,11 @@ def ln_linear(x, W, gamma, beta, bias=None, pe=None, hw=1, frames=1, mode=EPI_LI
     return out
 
 
-def linear_ln_linear(x0, W0, b0, W, gamma, beta, residual=None, bias=None, mode=EPI_LINEAR):
-    """x = x0 @ W0^T + b0 (+ residual) [fp16]; out = LayerNorm(x) @ W^T + bias (or GEGLU), the LayerNorm's row statistics
-    coming from the first GEMM's epilogue.  Returns (x, out)."""
+def linear_ln_linear(x0, W0, b0, W, gamma, beta, residual=None, bias=None, mode=EPI_LINEAR, pe=None, hw=1, frames=1):
+    """x = x0 @ W0^T + b0 (+ residual) [fp16]; out = (LayerNorm(x) (+ pe[(row // hw) % frames])) @ W^T + bias (or GEGLU),
+    the LayerNorm's row statistics coming from the first GEMM's epilogue.  Returns (x, out)."""
     _chk16(x0, W0, W, residual)
-    _chk32(b0, gamma, beta, bias)
+    _chk32(b0, gamma, beta, bias, pe)
     M, K0 = x0.shape
     Cc, N = W0.shape[0], W.shape[0]
     dev = x0.device
@@ -159,11 +233,13 @@ def linear_ln_linear(x0, W0, b0, W, gamma, beta, residual=None, bias=None, mode=
     wf = torch.empty_like(W)
     u = torch.empty((N,), dtype=torch.float32, device=dev)
     c = torch.empty((N,), dtype=torch.float32, device=dev)
+    cpe = torch.empty((pe.shape[0], N), dtype=torch.float32, device=dev) if pe is not None else None
     cap = 16
     parts = torch.empty((cap, M, 2), dtype=torch.float32, device=dev)
     out = torch.empty((M, N // 2 if mode == EPI_GEGLU else N), dtype=torch.float16, device=dev)
     _lib.call("vs_linear_ln_linear", _stream(), _p(x0), M, K0, _p(W0), _p(b0), _p(residual), Cc, _p(x), _p(W), _p(bias), N,
-              _p(gamma), _p(beta), mode, _p(wf), _p(u), _p(c), _p(parts), cap, _p(out))
+              _p(gamma), _p(beta), _p(pe), 0 if pe is None else pe.shape[0], hw, frames, mode, _p(wf), _p(u), _p(c), _p(cpe),
+              _p(parts), cap, _p(out))
     return x, out
 
 
@@ -210,13 +286,22 @@ def temporal_attention(qkv, heads):
     return out
 
 
-def conv_in(x, w, bias):
+def conv_in(x, w, bias, scratch="alloc"):
+    """conv_in (3x3, pad 1): x [N, H, W, ci], w [co, ci, 3, 3] -> [N, H, W, co].  By default (ci == 4) patch rows + the
+    tensor-core GEMM in a scratch buffer of (N H W + co) * 64 halves, as the UNet forward runs it; scratch=None selects
+    the direct CUDA-core kernel (also used for ci != 4)."""
     _chk16(x, w)
     _chk32(bias)
     n, H, W, ci = x.shape
     co = w.shape[0]
+    if isinstance(scratch, str):
+        assert scratch == "alloc"
+        scratch = torch.empty(((n * H * W + co) * 64,), dtype=torch.float16, device=x.device) if ci == 4 else None
+    _chk16(scratch)
+    if scratch is not None:
+        assert scratch.numel() >= (n * H * W + co) * 64
     out = torch.empty((n, H, W, co), dtype=torch.float16, device=x.device)
-    _lib.call("vs_conv_in", _stream(), _p(x), n, H, W, ci, _p(w), _p(bias), co, _p(out))
+    _lib.call("vs_conv_in", _stream(), _p(x), n, H, W, ci, _p(w), _p(bias), co, _p(scratch), _p(out))
     return out
 
 
