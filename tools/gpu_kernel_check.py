@@ -1,5 +1,6 @@
-"""GPU diagnostics: runs every kernel check in its own subprocess (a trapping kernel poisons the CUDA
-context, so isolation keeps the other results); REPORT_JSON = path of a JSON report."""
+"""GPU diagnostics: runs every kernel check (tests/kernel_checks.py and tests/test_attention_tc_gpu.py) in its own
+subprocess (a trapping kernel poisons the CUDA context, so isolation keeps the other results); REPORT_JSON = path of a
+JSON report."""
 import json
 import os
 import subprocess
@@ -9,17 +10,21 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
+def _checks():
+    from tests.kernel_checks import CHECKS
+    from tests.test_attention_tc_gpu import CASES      # the attention kernel's pipeline edge cases
+    return {**CHECKS, **CASES}
+
+
 def run_one(name):
     import torch
-    from tests.kernel_checks import CHECKS
-    r = CHECKS[name]()
+    r = _checks()[name]()
     torch.cuda.synchronize()
     print("RESULT " + json.dumps(r))
 
 
 def main():
-    from tests.kernel_checks import CHECKS
-    names = sys.argv[1:] or sorted(CHECKS)
+    names = sys.argv[1:] or sorted(_checks())
     out = {}
     for n in names:
         try:

@@ -216,20 +216,9 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128_mn(uint32_t smem_addr, uint3
 }
 
 #define VS_R8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-// m64n64k16: 32 fp32 accumulators per thread.  Register i holds row 16 w + lane / 4 + 8 ((i >> 1) & 1) of the warpgroup's
-// 64 rows (w = warp in the warpgroup) and column 8 (i >> 2) + 2 (lane & 3) + (i & 1).  tnspB = 1: B is MN-major.
-template <int TB = 0>
-__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-      "%32, %33, p, 1, 1, 0, %35;\n\t}"
-      : VS_R8(0), VS_R8(8), VS_R8(16), VS_R8(24)
-      : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
-}
-// m64nNk16 with both operands K-major in shared memory: one instruction for the full width of a GEMM tile (N / 2
-// accumulators per thread, in the register layout of wgmma_m64n64 extended to N columns).
+// m64nNk16 with both operands K-major in shared memory: one instruction for the full width of a tile, N / 2 fp32
+// accumulators per thread.  Register i holds row 16 w + lane / 4 + 8 ((i >> 1) & 1) of the warpgroup's 64 rows (w = warp
+// in the warpgroup) and column 8 (i >> 2) + 2 (lane & 3) + (i & 1).
 template <int N>
 __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t scale_d);
 #define VS_REGS_0_31 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
@@ -266,7 +255,8 @@ __device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t da, uint64_t db,
       : VS_R8(0)
       : "l"(da), "l"(db), "r"(scale_d), "n"(TB));
 }
-// A from registers (four fp16x2 per thread in the m16n8k16 A-fragment layout of each warp's 16 rows), B from smem.
+// A from registers (four fp16x2 per thread in the m16n8k16 A-fragment layout of each warp's 16 rows), B from smem;
+// tnspB (TB) = 1: B is MN-major.
 template <int TB = 0>
 __device__ __forceinline__ void wgmma_m64n64_rs(float* d, const uint32_t* a, uint64_t db, uint32_t scale_d) {
   asm volatile(
