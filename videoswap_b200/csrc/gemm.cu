@@ -2,20 +2,26 @@
 //
 // One persistent, warp-specialised kernel of three warpgroups: warpgroup 0 is the TMA producer (one elected thread of
 // warp 0 issues the copies; the warpgroup gives most of its registers to the others with setmaxnreg), warpgroups 1 and 2
-// are ping-pong consumers.  A tile is 64 (M) x BN (N); the tiles of a CTA alternate between the two consumers, each of
-// which issues one full-width wgmma.m64nBNk16 per k16 step on the 128-byte-swizzled operand ring in shared memory and
-// keeps its accumulator in registers.  Two named barriers hand the tensor cores from one consumer to the other once its
-// MMAs are issued, so one consumer's epilogue runs under the other's main loop.  A CTA walks 128-row x BN units whose
-// two 64-row halves go to the two consumers back to back: the second load of the weight tile hits L2.  K advances 64
-// elements (one swizzle row of fp16) per ring stage; the producer fills the ring in the order the consumers take the
-// tiles and runs up to STAGES k-blocks ahead, across tile boundaries.
+// are the consumers.  A tile is 128 (M) x BN (N); a ring stage holds its 128 x 64 A box and one BN x 64 weight box, so
+// each weight tile is brought into shared memory once per 128 rows.  The consumers issue full-width wgmma.m64nBNk16 on
+// the 128-byte-swizzled ring and keep their accumulators in registers; how they share the tiles is fixed by BN:
+//  * ping-pong (BN <= 160): the CTA's tiles alternate between the two consumers; a consumer owns the whole 128 x BN tile
+//    and issues two m64 MMAs per k16 step (A rows 0-63 and 64-127, the same weight descriptor), BN accumulators a
+//    thread.  Two named barriers hand the tensor cores from one consumer to the other once its MMAs are issued, so one
+//    consumer's epilogue runs under the other's main loop.
+//  * cooperative (BN = 256): both consumers work on every tile, consumer g on rows 64 g .. 64 g + 63 (128 accumulators a
+//    thread); a stage is free once all 8 consumer warps have read it.  Epilogues do not overlap MMAs.
+// Tiles are (m_tile, n_tile), n fastest, round-robin over the persistent CTAs.  K advances 64 elements (one swizzle row
+// of fp16) per ring stage; the producer fills the ring in the order the consumers take the tiles and runs up to STAGES
+// k-blocks ahead, across tile boundaries.
 // A 3x3 convolution is the same kernel with nine K segments: tap (dy,dx) loads the NHWC activation box shifted by
 // (dy,dx) through a 4-D TMA descriptor and the out-of-bounds zero fill of TMA provides the padding; a channel concat
 // is two descriptors walked back to back along K.
 //
-// Epilogue (per consumer warp, 16 rows): registers -> [folded LayerNorm: rstd * acc - rstd * mean * u] + bias (+ time-
-// embedding / positional row vector) / GEGLU -> fp16 -> warp-private swizzled shared-memory transpose, 32 columns at a
-// time -> (+ fp16 residual) -> coalesced 16-byte global stores.  Tiny-N outputs (conv_out, N = 4) keep a direct-store path.
+// Epilogue (per consumer warp, 16 rows of each 64-row half, one half after the other): registers -> [folded LayerNorm:
+// rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU -> fp16 -> warp-private
+// swizzled shared-memory transpose, 32 columns at a time -> (+ fp16 residual) -> coalesced 16-byte global stores.
+// Tiny-N outputs (conv_out, N = 4) keep a direct-store path.
 //
 // Replaces (reference call sites): InflatedConv3d 3x3 / 1x1 (models/animatediff_models/resnet.py:9-18), every
 // nn.Linear / 1x1 conv of Transformer3DModel (attention.py:65-93,174-204) and the motion module
@@ -27,9 +33,11 @@ namespace vs {
 
 namespace {
 
-constexpr int BM = 64;                              // rows of a tile (= of one consumer warpgroup)
+constexpr int BM = 128;                             // rows of a tile
+constexpr int WG_M = 64;                            // rows of one wgmma.m64 (an accumulator half)
 constexpr int BK = 64;
-constexpr int A_STAGE_BYTES = BM * BK * 2;          // 8 KB
+constexpr int A_STAGE_BYTES = BM * BK * 2;          // 16 KB
+constexpr uint64_t A_HALF_DESC = (WG_M * BK * 2) >> 4;   // descriptor step from A rows 0..63 to rows 64..127 (8 KB)
 constexpr int GEMM_THREADS = 384;                   // producer warpgroup + 2 consumer warpgroups
 constexpr int SMEM_LIMIT = 227 * 1024;
 constexpr int EPI_COLS = 32;                        // output columns per epilogue sub-tile (64 B of fp16)
@@ -72,6 +80,10 @@ struct GemmParams {
 
 template <int BN>
 struct Cfg {
+  // Cooperative (both consumers on one 128 x BN tile, 64 rows each) for BN = 256: 128 accumulators a thread.  Ping-pong
+  // (one consumer owns the whole tile: two m64 halves, BN accumulators a thread) for the narrower tiles.
+  static constexpr bool COOP = BN > 160;
+  static constexpr int HALVES = COOP ? 1 : 2;       // 64-row accumulator halves per consumer
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
@@ -110,15 +122,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
   const int nst = (p.stages > 0 && p.stages < C::STAGES) ? p.stages : C::STAGES;   // ring depth (debug knob: "gemm_stages")
-  // Tile order: units of (two 64-row tiles) x (one column tile), n fastest, round-robin over the CTAs (CTAs running at
-  // the same time share the A row panel and a few weight tiles in L2); the halves of a unit are consecutive tiles of the
-  // CTA and so go to the two consumers.
-  const int total_units = ((p.m_tiles + 1) >> 1) * p.n_tiles;
-  auto next_tile = [&](int& u, int& h) {       // (unit u, half h) -> the CTA's next tile; u >= total_units at the end
-    if (h == 0 && 2 * (u / p.n_tiles) + 1 < p.m_tiles) { h = 1; return; }
-    h = 0;
-    u += gridDim.x;
-  };
+  // Tile order: tile t = (m_tile, n_tile) = (t / n_tiles, t % n_tiles), n fastest, round-robin over the CTAs (CTAs
+  // running at the same time share the A row panel and a few weight tiles in L2).
+  const int total_tiles = p.m_tiles * p.n_tiles;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&p.tmA);
@@ -126,7 +132,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     if (p.kb_src1 < p.kb_per_tap) prefetch_tmap(&p.tmA2);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 4);                // one arrival per warp of the consumer that read the stage
+      mbar_init(empty_bar(s), C::COOP ? 8 : 4);  // one arrival per warp of the consumer(s) that read the stage
     }
     fence_barrier_init();
   }
@@ -142,8 +148,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     const bool conv = p.a_rank == 4;
     const int tap_x0 = p.tap_x0, tap_x1 = p.tap_x0 + p.tap_w;
     uint32_t pr_s = 0, pr_ph = 0;              // ring stage / phase, carried across tiles
-    for (int u = blockIdx.x, h = 0; u < total_units; next_tile(u, h)) {
-      const int m_tile = 2 * (u / p.n_tiles) + h, n_tile = u % p.n_tiles;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+      const int m_tile = t / p.n_tiles, n_tile = t % p.n_tiles;
       int x0 = 0, y0 = 0, i0 = 0;
       if (conv) {
         x0 = (m_tile % p.tiles_x) * p.TW;
@@ -182,10 +188,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 
   // ===================================================================== consumers: MMA + epilogue
   setmaxnreg_inc<CONSUMER_REGS>();
-  const int g = wg - 1;                        // consumer g takes the CTA's tiles j with j % 2 == g
-  const int wq = warp & 3;                     // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of the tile
+  const int g = wg - 1;                        // ping-pong: consumer g takes the CTA's tiles j with j % 2 == g;
+                                               // cooperative: consumer g takes rows 64 g .. 64 g + 63 of every tile
+  const int wq = warp & 3;                     // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of a 64-row half
   const int q = lane & 3;
-  const int rbase = 16 * wq + (lane >> 2);     // this thread's tile rows: rbase and rbase + 8
+  const int rbase = 16 * wq + (lane >> 2);     // this thread's rows of a half: rbase and rbase + 8
   const uint32_t stage_buf = epi_base + (uint32_t)(warp - 4) * EPI_WARP_BYTES;
   const bool has_bias = p.bias != nullptr;
   const bool staged = p.staged != 0;
@@ -204,31 +211,35 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     return px < p.M ? px : -1;
   };
 
-  // Tensor-core hand-off: consumer g waits on named barrier 1 + g before its main loop and, once all MMAs of its tile are
-  // issued, arrives on the other consumer's barrier -- only when the CTA has a next tile, so every arrival is waited for.
+  // Ping-pong tensor-core hand-off: consumer g waits on named barrier 1 + g before its main loop and, once all MMAs of
+  // its tile are issued, arrives on the other consumer's barrier -- only when the CTA has a next tile, so every arrival
+  // is waited for.  The cooperative consumers share every tile and need no hand-off.
   const int bar_mine = 1 + g, bar_other = 2 - g;
-  float acc[BN / 2];
+  float acc[C::HALVES][BN / 2];
   uint32_t s = 0, ph = 0;                      // ring stage / phase of the next tile's first k-block
-  for (int u = blockIdx.x, h = 0, j = 0; u < total_units; ++j) {
-    const int m_tile = 2 * (u / p.n_tiles) + h, n_tile = u % p.n_tiles;
-    next_tile(u, h);
-    if ((j & 1) != g) {                        // the other consumer's tile: skip its k-blocks in the ring
-      const uint32_t t = s + (uint32_t)num_kb;
-      ph ^= (t / (uint32_t)nst) & 1u;
-      s = t % (uint32_t)nst;
+  for (int t = blockIdx.x, j = 0; t < total_tiles; t += gridDim.x, ++j) {
+    const int m_tile = t / p.n_tiles, n_tile = t % p.n_tiles;
+    if (!C::COOP && (j & 1) != g) {            // the other consumer's tile: skip its k-blocks in the ring
+      const uint32_t sn = s + (uint32_t)num_kb;
+      ph ^= (sn / (uint32_t)nst) & 1u;
+      s = sn % (uint32_t)nst;
       continue;
     }
     // ------------------------------------------------------------------ main loop
-    if (j > 0) named_bar_sync(bar_mine, 256);
+    if (!C::COOP && j > 0) named_bar_sync(bar_mine, 256);
     uint32_t prev = 0;
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(full_bar(s), ph);
       wgmma_fence();
       const uint32_t a_addr = smem_base + s * C::STAGE_BYTES;
-      const uint64_t da = gmma_desc_sw128(a_addr);
+      const uint64_t da = gmma_desc_sw128(a_addr) + (C::COOP ? (uint64_t)g * A_HALF_DESC : 0);
       const uint64_t db = gmma_desc_sw128(a_addr + A_STAGE_BYTES);
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, da + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      for (int k = 0; k < BK / 16; ++k) {
+#pragma unroll
+        for (int hh = 0; hh < C::HALVES; ++hh)  // both m64 halves read the same weight tile
+          wgmma_ss<BN>(acc[hh], da + hh * A_HALF_DESC + 2 * k, db + 2 * k, (kb | k) != 0 ? 1u : 0u);
+      }
       wgmma_commit();
       if (kb > 0) {                            // the MMAs of the previous k-block have read their stage: release it
         wgmma_wait<1>();
@@ -237,154 +248,158 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       prev = s;
       if (++s == (uint32_t)nst) { s = 0; ph ^= 1; }
     }
-    if (u < total_units) named_bar_arrive(bar_other, 256);
+    if (!C::COOP && t + (int)gridDim.x < total_tiles) named_bar_arrive(bar_other, 256);
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(empty_bar(prev));
 
-    // ------------------------------------------------------------------ epilogue
+    // ------------------------------------------------------------------ epilogue, one 64-row half at a time
     const int n0 = n_tile * BN;
-    int pix[2];
-    pix[0] = tile_pixel(m_tile, rbase);
-    pix[1] = tile_pixel(m_tile, rbase + 8);
-    const float* rv[2] = {nullptr, nullptr};
-    if (HAS_RV || !staged) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (p.rowvec != nullptr && pix[h] >= 0) {
-          int ri = pix[h] / p.pix_per_batch;
-          if (p.rv_mod > 0) ri %= p.rv_mod;
-          rv[h] = p.rowvec + (long long)ri * p.ldrv + n0;
-        }
-      }
-    }
-    if (staged) {
-      constexpr int OC = GEGLU ? BN / 2 : BN;                            // output columns of a full tile
-      const int oc0 = n_tile * OC;                                        // first output column of this tile
-      const int nsub = (p.N - n0 < BN ? (GEGLU ? (p.N - n0) / 2 : p.N - n0) : OC) / EPI_COLS;
-      float la[2] = {1.f, 1.f}, lb[2] = {0.f, 0.f};                      // folded LayerNorm: row scale and shift factor
-      if (LN) {
+    for (int hh = 0; hh < C::HALVES; ++hh) {
+      const int r0 = WG_M * (C::COOP ? g : hh) + rbase;   // tile rows of this thread: r0 and r0 + 8
+      int pix[2];
+      pix[0] = tile_pixel(m_tile, r0);
+      pix[1] = tile_pixel(m_tile, r0 + 8);
+      const float* rv[2] = {nullptr, nullptr};
+      if (HAS_RV || !staged) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (pix[h] < 0) continue;
-          if (p.ln_nparts > 0) {            // statistics from the producer GEMM's per-column-tile partial sums
-            float S = 0.f, Q = 0.f;
-            for (int k = 0; k < p.ln_nparts; ++k) {
-              const float2 v = __ldg(p.ln_parts + (long long)k * p.M + pix[h]);
-              S += v.x; Q += v.y;
-            }
-            const float mean = S * p.ln_inv_c;
-            la[h] = rsqrtf(fmaxf(fmaf(-mean, mean, Q * p.ln_inv_c), 0.f) + 1e-5f);
-            lb[h] = -mean * la[h];
-          } else {
-            const float2 st2 = __ldg(p.ln_stats + pix[h]);
-            la[h] = st2.x; lb[h] = st2.y;
+          if (p.rowvec != nullptr && pix[h] >= 0) {
+            int ri = pix[h] / p.pix_per_batch;
+            if (p.rv_mod > 0) ri %= p.rv_mod;
+            rv[h] = p.rowvec + (long long)ri * p.ldrv + n0;
           }
         }
       }
-      float rs[2] = {0.f, 0.f}, rq[2] = {0.f, 0.f};   // LNOUT: sums of the 2 rows this lane stores
-      // After the transpose this lane stores 16-byte chunk q of its own two rows (rbase, rbase + 8).
-      __half* orow[2];
-      const __half* rrow[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long long px = pix[h] >= 0 ? pix[h] : 0;     // rows outside the problem: loads harmless, stores predicated
-        orow[h] = p.out + px * p.ldc + oc0 + q * 8;
-        rrow[h] = HAS_RES ? p.residual + px * p.ldr + oc0 + q * 8 : nullptr;
-      }
-#pragma unroll
-      for (int sb = 0; sb < OC / EPI_COLS; ++sb) {
-        if (sb >= nsub) break;                  // warp-uniform
-        uint4 rr[2];
-        if (HAS_RES) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) rr[h] = __ldg(reinterpret_cast<const uint4*>(rrow[h] + sb * EPI_COLS));
-        }
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int j = 4 * sb + jj;            // n8 block of the (output) tile
-          const int c = 8 * j + 2 * q;          // column inside the tile (value column for GEGLU)
-          float2 b = has_bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
-          float2 u = LN ? __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + c)) : make_float2(0.f, 0.f);
-          float2 bg = make_float2(0.f, 0.f), ug = make_float2(0.f, 0.f);
-          if (GEGLU) {                          // gate columns are BN / 2 further on, in the same thread's registers
-            bg = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + BN / 2 + c));
-            if (LN) ug = __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + BN / 2 + c));
-          }
+      if (staged) {
+        constexpr int OC = GEGLU ? BN / 2 : BN;                            // output columns of a full tile
+        const int oc0 = n_tile * OC;                                        // first output column of this tile
+        const int nsub = (p.N - n0 < BN ? (GEGLU ? (p.N - n0) / 2 : p.N - n0) : OC) / EPI_COLS;
+        float la[2] = {1.f, 1.f}, lb[2] = {0.f, 0.f};                      // folded LayerNorm: row scale and shift factor
+        if (LN) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-            if (GEGLU) {
-              float g0 = acc[4 * (j + BN / 16) + 2 * h], g1 = acc[4 * (j + BN / 16) + 2 * h + 1];
-              float bv0 = b.x, bv1 = b.y, bg0 = bg.x, bg1 = bg.y;
-              if (LN) {                         // value / gate pre-activations of the folded LayerNorm
-                bv0 = fmaf(lb[h], u.x, bv0); bv1 = fmaf(lb[h], u.y, bv1);
-                bg0 = fmaf(lb[h], ug.x, bg0); bg1 = fmaf(lb[h], ug.y, bg1);
-                f0 *= la[h]; f1 *= la[h]; g0 *= la[h]; g1 *= la[h];
+            if (pix[h] < 0) continue;
+            if (p.ln_nparts > 0) {            // statistics from the producer GEMM's per-column-tile partial sums
+              float S = 0.f, Q = 0.f;
+              for (int k = 0; k < p.ln_nparts; ++k) {
+                const float2 v = __ldg(p.ln_parts + (long long)k * p.M + pix[h]);
+                S += v.x; Q += v.y;
               }
-              f0 = (f0 + bv0) * gelu_sig(g0 + bg0);
-              f1 = (f1 + bv1) * gelu_sig(g1 + bg1);
+              const float mean = S * p.ln_inv_c;
+              la[h] = rsqrtf(fmaxf(fmaf(-mean, mean, Q * p.ln_inv_c), 0.f) + 1e-5f);
+              lb[h] = -mean * la[h];
             } else {
-              if (LN) {                         // rstd * acc + (-mean rstd) * u + c in two FMAs per element
-                f0 = fmaf(la[h], f0, fmaf(lb[h], u.x, b.x));
-                f1 = fmaf(la[h], f1, fmaf(lb[h], u.y, b.y));
-              } else if (has_bias) {
-                f0 += b.x; f1 += b.y;
-              }
-              if (HAS_RV && rv[h] != nullptr) {
-                const float2 r2 = __ldg(reinterpret_cast<const float2*>(rv[h] + c));
-                f0 += r2.x; f1 += r2.y;
-              }
+              const float2 st2 = __ldg(p.ln_stats + pix[h]);
+              la[h] = st2.x; lb[h] = st2.y;
             }
-            const __half2 hv = __floats2half2_rn(f0, f1);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(stage_buf + sw64_off((lane >> 2) + 8 * h, jj) + 4 * q),
-                         "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
           }
         }
-        __syncwarp();
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {           // 8 rows x 64 contiguous bytes per store instruction
-          uint4 o;
-          asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
-                       : "r"(stage_buf + sw64_off((lane >> 2) + 8 * h, q)));
-          if (HAS_RES) {                        // fp16 add: the rounding order of the reference's `linear(x) + residual`
-            __half2* oh = reinterpret_cast<__half2*>(&o);
-            const __half2* rh = reinterpret_cast<const __half2*>(&rr[h]);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) oh[t] = __hadd2(oh[t], rh[t]);
-          }
-          if (pix[h] >= 0) *reinterpret_cast<uint4*>(orow[h] + sb * EPI_COLS) = o;
-          if (LNOUT) {
-            const __half2* oh = reinterpret_cast<const __half2*>(&o);
-            const float2 a = __half22float2(oh[0]), b2 = __half22float2(oh[1]), c2 = __half22float2(oh[2]), d2 = __half22float2(oh[3]);
-            rs[h] += ((a.x + a.y) + (b2.x + b2.y)) + ((c2.x + c2.y) + (d2.x + d2.y));
-            float q0 = fmaf(a.x, a.x, a.y * a.y), q1 = fmaf(b2.x, b2.x, b2.y * b2.y);
-            float q2 = fmaf(c2.x, c2.x, c2.y * c2.y), q3 = fmaf(d2.x, d2.x, d2.y * d2.y);
-            rq[h] += (q0 + q1) + (q2 + q3);
-          }
-        }
-        __syncwarp();                           // staging buffer free for the next sub-tile
-      }
-      if (LNOUT) {                              // the 4 column chunks of a row sit in 4 adjacent lanes
+        float rs[2] = {0.f, 0.f}, rq[2] = {0.f, 0.f};   // LNOUT: sums of the 2 rows this lane stores
+        // After the transpose this lane stores 16-byte chunk q of its own two rows (rbase, rbase + 8).
+        __half* orow[2];
+        const __half* rrow[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 1); rq[h] += __shfl_xor_sync(0xffffffffu, rq[h], 1);
-          rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 2); rq[h] += __shfl_xor_sync(0xffffffffu, rq[h], 2);
-          if (q == 0 && pix[h] >= 0) p.ln_sums_out[(long long)n_tile * p.M + pix[h]] = make_float2(rs[h], rq[h]);
+          const long long px = pix[h] >= 0 ? pix[h] : 0;     // rows outside the problem: loads harmless, stores predicated
+          orow[h] = p.out + px * p.ldc + oc0 + q * 8;
+          rrow[h] = HAS_RES ? p.residual + px * p.ldr + oc0 + q * 8 : nullptr;
         }
-      }
-    } else {
-      // -------------------------------------------------------------- direct stores (tiny / unaligned N, linear only)
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
+        for (int sb = 0; sb < OC / EPI_COLS; ++sb) {
+          if (sb >= nsub) break;                  // warp-uniform
+          uint4 rr[2];
+          if (HAS_RES) {
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int h = e >> 1, c = 8 * j + 2 * q + (e & 1), n = n0 + c;
-          if (n < p.N && pix[h] >= 0) {
-            float f = acc[4 * j + e];
-            if (has_bias) f += p.bias[n];
-            if (rv[h]) f += rv[h][c];
-            if (p.residual) f += __half2float(p.residual[(long long)pix[h] * p.ldr + n]);
-            p.out[(long long)pix[h] * p.ldc + n] = __float2half_rn(f);
+            for (int h = 0; h < 2; ++h) rr[h] = __ldg(reinterpret_cast<const uint4*>(rrow[h] + sb * EPI_COLS));
+          }
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * sb + jj;            // n8 block of the (output) tile
+            const int c = 8 * j + 2 * q;          // column inside the tile (value column for GEGLU)
+            float2 b = has_bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
+            float2 u = LN ? __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + c)) : make_float2(0.f, 0.f);
+            float2 bg = make_float2(0.f, 0.f), ug = make_float2(0.f, 0.f);
+            if (GEGLU) {                          // gate columns are BN / 2 further on, in the same thread's registers
+              bg = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + BN / 2 + c));
+              if (LN) ug = __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + BN / 2 + c));
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float f0 = acc[hh][4 * j + 2 * h], f1 = acc[hh][4 * j + 2 * h + 1];
+              if (GEGLU) {
+                float g0 = acc[hh][4 * (j + BN / 16) + 2 * h], g1 = acc[hh][4 * (j + BN / 16) + 2 * h + 1];
+                float bv0 = b.x, bv1 = b.y, bg0 = bg.x, bg1 = bg.y;
+                if (LN) {                         // value / gate pre-activations of the folded LayerNorm
+                  bv0 = fmaf(lb[h], u.x, bv0); bv1 = fmaf(lb[h], u.y, bv1);
+                  bg0 = fmaf(lb[h], ug.x, bg0); bg1 = fmaf(lb[h], ug.y, bg1);
+                  f0 *= la[h]; f1 *= la[h]; g0 *= la[h]; g1 *= la[h];
+                }
+                f0 = (f0 + bv0) * gelu_sig(g0 + bg0);
+                f1 = (f1 + bv1) * gelu_sig(g1 + bg1);
+              } else {
+                if (LN) {                         // rstd * acc + (-mean rstd) * u + c in two FMAs per element
+                  f0 = fmaf(la[h], f0, fmaf(lb[h], u.x, b.x));
+                  f1 = fmaf(la[h], f1, fmaf(lb[h], u.y, b.y));
+                } else if (has_bias) {
+                  f0 += b.x; f1 += b.y;
+                }
+                if (HAS_RV && rv[h] != nullptr) {
+                  const float2 r2 = __ldg(reinterpret_cast<const float2*>(rv[h] + c));
+                  f0 += r2.x; f1 += r2.y;
+                }
+              }
+              const __half2 hv = __floats2half2_rn(f0, f1);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(stage_buf + sw64_off((lane >> 2) + 8 * h, jj) + 4 * q),
+                           "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
+            }
+          }
+          __syncwarp();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {           // 8 rows x 64 contiguous bytes per store instruction
+            uint4 o;
+            asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                         : "r"(stage_buf + sw64_off((lane >> 2) + 8 * h, q)));
+            if (HAS_RES) {                        // fp16 add: the rounding order of the reference's `linear(x) + residual`
+              __half2* oh = reinterpret_cast<__half2*>(&o);
+              const __half2* rh = reinterpret_cast<const __half2*>(&rr[h]);
+#pragma unroll
+              for (int t = 0; t < 4; ++t) oh[t] = __hadd2(oh[t], rh[t]);
+            }
+            if (pix[h] >= 0) *reinterpret_cast<uint4*>(orow[h] + sb * EPI_COLS) = o;
+            if (LNOUT) {
+              const __half2* oh = reinterpret_cast<const __half2*>(&o);
+              const float2 a = __half22float2(oh[0]), b2 = __half22float2(oh[1]), c2 = __half22float2(oh[2]), d2 = __half22float2(oh[3]);
+              rs[h] += ((a.x + a.y) + (b2.x + b2.y)) + ((c2.x + c2.y) + (d2.x + d2.y));
+              float q0 = fmaf(a.x, a.x, a.y * a.y), q1 = fmaf(b2.x, b2.x, b2.y * b2.y);
+              float q2 = fmaf(c2.x, c2.x, c2.y * c2.y), q3 = fmaf(d2.x, d2.x, d2.y * d2.y);
+              rq[h] += (q0 + q1) + (q2 + q3);
+            }
+          }
+          __syncwarp();                           // staging buffer free for the next sub-tile
+        }
+        if (LNOUT) {                              // the 4 column chunks of a row sit in 4 adjacent lanes
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 1); rq[h] += __shfl_xor_sync(0xffffffffu, rq[h], 1);
+            rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 2); rq[h] += __shfl_xor_sync(0xffffffffu, rq[h], 2);
+            if (q == 0 && pix[h] >= 0) p.ln_sums_out[(long long)n_tile * p.M + pix[h]] = make_float2(rs[h], rq[h]);
+          }
+        }
+      } else {
+        // -------------------------------------------------------------- direct stores (tiny / unaligned N, linear only)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int h = e >> 1, c = 8 * j + 2 * q + (e & 1), n = n0 + c;
+            if (n < p.N && pix[h] >= 0) {
+              float f = acc[hh][4 * j + e];
+              if (has_bias) f += p.bias[n];
+              if (rv[h]) f += rv[h][c];
+              if (p.residual) f += __half2float(p.residual[(long long)pix[h] * p.ldr + n]);
+              p.out[(long long)pix[h] * p.ldc + n] = __float2half_rn(f);
+            }
           }
         }
       }
@@ -419,9 +434,9 @@ int launch(cudaStream_t st, const GemmParams& p) {
     VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
-  const int total = ((p.m_tiles + 1) / 2) * p.n_tiles;   // units of two tiles
+  const int total = p.m_tiles * p.n_tiles;
   int ctas = num_sms();
-  const int cap = get_option("gemm_ctas");              // > 0: fewer CTAs, each walking more units (another tile schedule)
+  const int cap = get_option("gemm_ctas");              // > 0: fewer CTAs, each walking more tiles (another tile schedule)
   if (cap > 0 && cap < ctas) ctas = cap;
   return launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(total < ctas ? total : ctas), dim3(GEMM_THREADS), C::SMEM_BYTES, st, 1, p);
 }
@@ -443,10 +458,10 @@ int launch_linear(cudaStream_t st, const GemmParams& p) {
   }
 }
 
-// BLOCK_N by a two-term model: waves of the persistent grid x operand bytes per k-block of one unit of two tiles
-// (2 x 8 KB of A + BN * 128 B of B; wider tiles need fewer bytes per flop).  Ties go to the wider tile only for long K,
-// where the main loop -- not the epilogue -- dominates.
-int pick_bn(int m_units, int N, int num_kb) {
+// BLOCK_N by a two-term model: waves of 128 x BN tiles over the persistent grid x operand bytes per k-block of one tile
+// (16 KB of A + BN * 128 B of B; wider tiles need fewer bytes per flop).  Ties go to the wider tile only for long K,
+// where the main loop -- not the epilogue -- dominates.  Never below 128 for N > 64 (ops.max_column_tiles relies on it).
+int pick_bn(int m_tiles, int N, int num_kb) {
   if (N <= 64) return 64;
   int best = 128;
   long long best_cost = -1;
@@ -454,8 +469,8 @@ int pick_bn(int m_units, int N, int num_kb) {
   for (int i = 0; i < 3; ++i) {
     const int bn = cand[i];
     if (bn != 128 && N % bn != 0) continue;
-    const long long units = (long long)m_units * ((N + bn - 1) / bn);
-    const long long waves = (units + num_sms() - 1) / num_sms();
+    const long long tiles = (long long)m_tiles * ((N + bn - 1) / bn);
+    const long long waves = (tiles + num_sms() - 1) / num_sms();
     const long long cost = waves * (16 + bn / 8);           // KB per k-block: 16 (A) + bn * 128 B (B)
     if (best_cost < 0 || cost < best_cost || (cost == best_cost && num_kb >= 40)) {
       best_cost = cost;
@@ -474,7 +489,7 @@ int gemm_n_tiles(const GemmArgs& a) {
   if (a.taps != 1) return 0;
   int bn = a.force_bn;
   if (a.mode == EPI_GEGLU) bn = 2 * kGegluGranule;
-  else if (bn == 0) bn = pick_bn((a.M + 2 * BM - 1) / (2 * BM), a.N, (a.K1 + BK - 1) / BK + a.K2 / BK);
+  else if (bn == 0) bn = pick_bn((a.M + BM - 1) / BM, a.N, (a.K1 + BK - 1) / BK + a.K2 / BK);
   return (a.N + bn - 1) / bn;
 }
 
@@ -567,7 +582,7 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
     VS_REQUIRE(a.N % bn == 0, "gemm_tc: GEGLU needs N %% %d == 0 (N=%d)", bn, a.N);
     VS_REQUIRE(a.bias != nullptr && a.residual == nullptr && a.rowvec == nullptr, "gemm_tc: GEGLU takes a bias only");
   } else if (bn == 0) {
-    bn = pick_bn((p.m_tiles + 1) / 2, a.N, p.num_kb);
+    bn = pick_bn(p.m_tiles, a.N, p.num_kb);
   }
   VS_REQUIRE(bn == 64 || bn == 128 || bn == 160 || bn == 256, "gemm_tc: unsupported BLOCK_N %d", bn);
   p.n_tiles = (a.N + bn - 1) / bn;
