@@ -66,7 +66,9 @@ const char* vs_unet_param_name(const vs_unet* h, int i);
  *   d_residuals 4 adapter maps (or NULL): NHWC fp16 [(B F), H_l, W_l, C_l] if residuals_nhwc else NCHW fp16
  *              [(B F), C_l, H_l, W_l] as the reference passes them (down_block_additional_residuals, unet.py:336);
  *              residual_scale multiplies them (t2i_guidance_scale, pipeline_videoswap.py:544-545)
- *   d_out      [B, C_out, F, H, W] same dtype as d_sample */
+ *   d_out      [B, C_out, F, H, W] same dtype as d_sample
+ * Any H, W >= 1 (unet.py:356-364,454-457): level l has H_l = ceil(H_(l-1) / 2) (the stride-2 convs) and every up-sampler
+ * targets the size of the skip it feeds; the adapter maps must have those level sizes. */
 int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
                     const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers,
                     const void* const* d_residuals, int residuals_nhwc, float residual_scale, void* d_out);
@@ -153,7 +155,9 @@ int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0, const voi
  * field the library's internal GEMM arguments; zero-initialise and set what is used).
  *   out[pix, n] = epilogue( sum_k [A | A2][pix (+ tap shift), k] * Bw[n, k] )
  *   taps 1: A [M, K1] (row stride lda1) (+ A2 [M, K2], lda2, channel concat along K); taps 9: NHWC [nimg, H, W, K1] 3x3
- *   convolution, pad 1 (M = nimg H W); taps 4: one output parity (sub_py, sub_px) of nearest-2x + 3x3.  Bw [N, taps (K1 + K2)].
+ *   convolution, pad 1 (M = nimg H W); taps 4: one output parity (sub_py, sub_px) of nearest-2x + 3x3 into an OH x OW output
+ *   (OH = 2H or 2H - 1, OW = 2W or 2W - 1; 0 = 2H / 2W).  Bw [N, taps (K1 + K2)], where taps = 4 except for parity 0 along
+ *   an odd output axis, which has 3 taps along it (6 or 9 in all; see vs_upsample_conv3x3_sized for the panels).
  *   Epilogue: + bias[n] + rowvec[((pix / pix_per_batch) % rv_mod if rv_mod > 0), n] (row stride ldrv, 0 = N) + residual[pix, n]
  *   (row stride ldr; may alias `out`); mode 1 = GEGLU on packed weights (N / 2 output columns).  Folded LayerNorm of A:
  *   ln_u [N] with ln_stats [M, 2] (rstd, -mean rstd) or ln_parts [ln_nparts][M][2] (sum, sum of squares).
@@ -176,6 +180,7 @@ typedef struct vs_gemm_desc {
   void* out; int ldc;
   int mode;
   int force_bn;
+  int OH, OW;
 } vs_gemm_desc;
 int vs_gemm_ex(void* stream, const vs_gemm_desc* desc);
 int vs_pack_conv3x3(void* stream, const void* d_w, int cout, int cin, void* d_out);
@@ -224,6 +229,15 @@ int vs_upsample2x(void* stream, const void* d_x, int nimg, int H, int W, int C, 
  * fp16 as in the state_dict; d_wsub: scratch for the 4 panels, 16 * Cout * C halves; d_out: NHWC [nimg, 2H, 2W, Cout]. */
 int vs_upsample_conv3x3(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w, int Cout,
                         const float* d_bias, void* d_wsub, void* d_out);
+/* The same to an explicit output size, as the UNet's up path runs it (the reference's forward_upsample_size path,
+ * unet.py:356-364,454-457): nearest up-sampling of [nimg, H, W, C] to OH x OW (OH = 2H or 2H - 1, OW = 2W or 2W - 1,
+ * torch's nearest: source row y / 2) then conv3x3.  Along an odd axis the last up-sampled row/column is padding, so
+ * parity 0 keeps its three weight taps apart.  d_wpanels: scratch for the packed panels, 49 * Cout * C halves (the 3x3
+ * panel, then the 40 taps of the sub-pixel panels); d_out: NHWC [nimg, OH, OW, Cout]. */
+int vs_upsample_conv3x3_sized(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w, int Cout,
+                              const float* d_bias, int OH, int OW, void* d_wpanels, void* d_out);
+/* Nearest up-sampling of NHWC [nimg, H, W, C] to [nimg, OH, OW, C] (OH in {2H - 1, 2H}, OW in {2W - 1, 2W}). */
+int vs_upsample_nearest(void* stream, const void* d_x, int nimg, int H, int W, int C, int OH, int OW, void* d_out);
 int vs_conv3x3_s2(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w_packed, int Cout,
                   const float* d_bias, void* d_scratch, void* d_out);
 

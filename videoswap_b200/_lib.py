@@ -54,6 +54,7 @@ class GemmDescStruct(C.Structure):
         ("out", _P), ("ldc", _I),
         ("mode", _I),
         ("force_bn", _I),
+        ("OH", _I), ("OW", _I),
     ]
 
 _SIGNATURES = {
@@ -108,6 +109,8 @@ _SIGNATURES = {
     "vs_conv_in": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _I, _P, _P]),
     "vs_upsample2x": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "vs_upsample_conv3x3": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P, _P]),
+    "vs_upsample_conv3x3_sized": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P]),
+    "vs_upsample_nearest": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "vs_conv3x3_s2": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P, _P]),
 }
 

@@ -57,6 +57,7 @@ extern "C" int vs_gemm_ex(void* stream, const vs_gemm_desc* d) {
   g.out = (__half*)d->out; g.ldc = d->ldc;
   g.mode = d->mode;
   g.force_bn = d->force_bn;
+  g.OH = d->OH; g.OW = d->OW;
   return gemm_tc((cudaStream_t)stream, g);
 }
 
@@ -123,6 +124,19 @@ extern "C" int vs_upsample_conv3x3(void* stream, const void* d_x, int nimg, int 
     if (int e = gemm_tc(st, g)) return e;
   }
   return 0;
+}
+extern "C" int vs_upsample_conv3x3_sized(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w, int Cout,
+                                         const float* d_bias, int OH, int OW, void* d_wpanels, void* d_out) {
+  cudaStream_t st = (cudaStream_t)stream;
+  VS_REQUIRE(d_x && d_w && d_wpanels && d_out && nimg >= 1 && H >= 1 && W >= 1, "vs_upsample_conv3x3_sized: bad arguments");
+  __half* w3x3 = (__half*)d_wpanels;
+  __half* wsub = w3x3 + (size_t)Cout * 9 * C;
+  if (int e = pack_conv3x3(st, (const __half*)d_w, Cout, C, w3x3)) return e;
+  if (int e = pack_conv_subpixel(st, (const __half*)d_w, Cout, C, wsub, true)) return e;
+  return upsample_conv3x3(st, (const __half*)d_x, nimg, H, W, C, w3x3, wsub, d_bias, Cout, OH, OW, (__half*)d_out);
+}
+extern "C" int vs_upsample_nearest(void* stream, const void* d_x, int nimg, int H, int W, int C, int OH, int OW, void* d_out) {
+  return upsample_nearest2x((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, C, (__half*)d_out, OH, OW);
 }
 extern "C" int vs_attention_probs(void* stream, const void* d_q, int ldq, const void* d_k, int ldk, void* d_probs, int batch, int nq,
                                   int nk, int heads, int d, long long q_bstride, long long kv_bstride, int kv_div) {

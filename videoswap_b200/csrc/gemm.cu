@@ -17,6 +17,12 @@
 // A 3x3 convolution is the same kernel with nine K segments: tap (dy,dx) loads the NHWC activation box shifted by
 // (dy,dx) through a 4-D TMA descriptor and the out-of-bounds zero fill of TMA provides the padding; a channel concat
 // is two descriptors walked back to back along K.
+// Nearest up-sampling + 3x3 conv runs as one launch per output parity on the low-resolution input (pack_conv_subpixel).
+// When the target size along an axis is odd (2n - 1, the up-sampler of a level whose size was odd on the way down),
+// parity 0 keeps the three row taps apart: its third tap reads the input through a descriptor whose base sits one row
+// (column) EARLIER, so coordinate y + 1 of that view is row y of the tensor and the last row falls off the end into the
+// zero fill -- which is exactly the padding the up-sampled image has below row 2n - 2.  Only coordinates >= 1 of such a
+// view are ever read.  Output pixels beyond the target extent (parity 1 on an odd axis) are never stored.
 //
 // Epilogue (per consumer warp, 16 rows of each 64-row half, one half after the other): registers -> [folded LayerNorm:
 // rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU -> fp16 -> warp-private
@@ -26,6 +32,8 @@
 // Replaces (reference call sites): InflatedConv3d 3x3 / 1x1 (models/animatediff_models/resnet.py:9-18), every
 // nn.Linear / 1x1 conv of Transformer3DModel (attention.py:65-93,174-204) and the motion module
 // (motion_module.py:113-136,202-218), GEGLU (diffusers FeedForward).
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -78,6 +86,13 @@ struct GemmParams {
   int stages;        // 0 = all, else limits the smem ring depth (pipeline-depth experiments)
 };
 
+// Sub-pixel conv to an odd-sized target (its own kernel instantiations, so every other launch keeps the parameter block
+// and the code it had): output extent check and the shifted views of the third tap along an odd axis.
+struct GemmParamsSub : GemmParams {
+  CUtensorMap tmS[3];    // tmA viewed one row (0), one column (1), one row and one column (2) earlier
+  int sub_short;         // bit 0 / 1: the third row / column tap of this parity reads through tmS
+};
+
 template <int BN>
 struct Cfg {
   // Cooperative (both consumers on one 128 x BN tile, 64 rows each) for BN = 256: 128 accumulators a thread.  Ping-pong
@@ -98,9 +113,10 @@ __device__ __forceinline__ uint32_t sw64_off(int row, int chunk) {   // byte off
   return (uint32_t)(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4));
 }
 
-template <int BN, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+template <int BN, int EPI, typename Params>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ Params p) {
   using C = Cfg<BN>;
+  constexpr bool SUB = std::is_same<Params, GemmParamsSub>::value;
   constexpr bool GEGLU = (EPI & EPI_F_GEGLU) != 0, HAS_RES = (EPI & EPI_F_RES) != 0, HAS_RV = (EPI & EPI_F_RV) != 0;
   // LN: the A operand is the RAW input of a LayerNorm whose affine map is folded into the weights:
   //   LN(x) W^T = rstd (x W'^T) - rstd mean u + c,  W' = W * gamma, u[n] = sum_k W'[n,k], c = beta W^T + bias (the `bias`)
@@ -130,6 +146,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     prefetch_tmap(&p.tmA);
     prefetch_tmap(&p.tmB);
     if (p.kb_src1 < p.kb_per_tap) prefetch_tmap(&p.tmA2);
+    if constexpr (SUB) {
+      if (p.sub_short & 1) prefetch_tmap(&p.tmS[0]);
+      if (p.sub_short & 2) prefetch_tmap(&p.tmS[1]);
+      if (p.sub_short == 3) prefetch_tmap(&p.tmS[2]);
+    }
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), C::COOP ? 8 : 4);  // one arrival per warp of the consumer(s) that read the stage
@@ -147,6 +168,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     const int num_kb = p.num_kb, kb_per_tap = p.kb_per_tap, kb_src1 = p.kb_src1;
     const bool conv = p.a_rank == 4;
     const int tap_x0 = p.tap_x0, tap_x1 = p.tap_x0 + p.tap_w;
+    bool short_y = false, short_x = false;
+    if constexpr (SUB) { short_y = (p.sub_short & 1) != 0; short_x = (p.sub_short & 2) != 0; }
     uint32_t pr_s = 0, pr_ph = 0;              // ring stage / phase, carried across tiles
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       const int m_tile = t / p.n_tiles, n_tile = t % p.n_tiles;
@@ -168,6 +191,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
           const uint32_t a_dst = smem_base + pr_s * C::STAGE_BYTES;
           const bool first = r < kb_src1;
           const CUtensorMap* tm = first ? &p.tmA : &p.tmA2;
+          if constexpr (SUB) {
+            const bool sy = short_y && dy == p.tap_y0 + 2, sx = short_x && dx == tap_x0 + 2;   // third tap of an odd axis
+            if (sy || sx) tm = sy ? (sx ? &p.tmS[2] : &p.tmS[0]) : &p.tmS[1];
+          }
           const int c = (first ? r : r - kb_src1) * BK;
           mbar_expect_tx(fb, C::STAGE_BYTES);
           if (conv) tma_load_4d(a_dst, tm, fb, c, x0 + dx, y0 + dy, i0);
@@ -205,6 +232,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       const int i0 = (m_tile / (p.tiles_x * p.tiles_y)) * p.TN;
       const int ti = row >> p.thw_log, rem = row & ((1 << p.thw_log) - 1);
       const int y = y0 + (rem >> p.tw_log), x = x0 + (rem & (p.TW - 1)), img = i0 + ti;
+      if constexpr (SUB) {                     // parity 1 of an odd axis: its last row / column is not stored
+        const int oy = y * p.osy + p.ooy, ox = x * p.osx + p.oox;
+        return ((img < p.nimg) && (y < p.H) && (x < p.W) && (oy < p.OH) && (ox < p.OW)) ? (img * p.OH + oy) * p.OW + ox : -1;
+      }
       return ((img < p.nimg) && (y < p.H) && (x < p.W)) ? (img * p.OH + y * p.osy + p.ooy) * p.OW + x * p.osx + p.oox : -1;
     }
     const int px = m_tile * BM + row;
@@ -426,19 +457,19 @@ ConvTile pick_conv_tile(int nimg, int H, int W) {   // BM pixels as a TW x TH x 
   return best;
 }
 
-template <int BN, int EPI>
-int launch(cudaStream_t st, const GemmParams& p) {
+template <int BN, int EPI, typename Params = GemmParams>
+int launch(cudaStream_t st, const Params& p) {
   using C = Cfg<BN>;
   static bool configured = false;
   if (!configured) {
-    VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, Params>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     configured = true;
   }
   const int total = p.m_tiles * p.n_tiles;
   int ctas = num_sms();
   const int cap = get_option("gemm_ctas");              // > 0: fewer CTAs, each walking more tiles (another tile schedule)
   if (cap > 0 && cap < ctas) ctas = cap;
-  return launch_pdl(gemm_tc_kernel<BN, EPI>, dim3(total < ctas ? total : ctas), dim3(GEMM_THREADS), C::SMEM_BYTES, st, 1, p);
+  return launch_pdl(gemm_tc_kernel<BN, EPI, Params>, dim3(total < ctas ? total : ctas), dim3(GEMM_THREADS), C::SMEM_BYTES, st, 1, p);
 }
 
 template <int BN>
@@ -495,19 +526,27 @@ int gemm_n_tiles(const GemmArgs& a) {
 
 int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   VS_REQUIRE(a.A && a.Bw && a.out, "gemm_tc: null pointer");
-  VS_REQUIRE(a.taps == 1 || a.taps == 9 || a.taps == 4, "gemm_tc: taps must be 1, 9 (3x3) or 4 (2x2 sub-pixel)");
+  VS_REQUIRE(a.taps == 1 || a.taps == 9 || a.taps == 4, "gemm_tc: taps must be 1, 9 (3x3) or 4 (sub-pixel)");
   VS_REQUIRE(a.K1 % 8 == 0 && a.K2 % 8 == 0, "gemm_tc: K must be a multiple of 8 (TMA 16-byte strides)");
   VS_REQUIRE((long long)a.M * (a.ldc > a.ldr ? a.ldc : a.ldr) < (1LL << 40) && a.M < (1 << 30), "gemm_tc: M too large");
   const bool two = a.A2 != nullptr && a.K2 > 0;
   if (two || a.taps != 1) VS_REQUIRE(a.K1 % BK == 0 && a.K2 % BK == 0, "gemm_tc: concat/conv sources need C %% 64 == 0 (got %d,%d)", a.K1, a.K2);
-  GemmParams p;
-  memset(&p, 0, sizeof(p));
+  GemmParamsSub ps;                            // the GemmParams part is what every launch but an odd-sized sub-pixel one takes
+  memset(&ps, 0, sizeof(ps));
+  GemmParams& p = ps;
+  // sub-pixel conv: output extent OH x OW (2H or 2H - 1 rows, 2W or 2W - 1 columns); parity 0 of an odd axis has 3 taps
+  const bool sub = a.taps == 4;
+  const int OH = sub && a.OH > 0 ? a.OH : 2 * a.H, OW = sub && a.OW > 0 ? a.OW : 2 * a.W;
+  const int sub_ty = sub && a.sub_py == 0 && (OH & 1) ? 3 : 2, sub_tx = sub && a.sub_px == 0 && (OW & 1) ? 3 : 2;
+  if (sub) VS_REQUIRE((OH == 2 * a.H || OH == 2 * a.H - 1) && (OW == 2 * a.W || OW == 2 * a.W - 1),
+                      "gemm_tc: sub-pixel output %dx%d is not 2x (or 2x - 1) of the %dx%d input", OH, OW, a.H, a.W);
+  const int ntaps = sub ? sub_ty * sub_tx : a.taps;
   const int Ktap = a.K1 + (two ? a.K2 : 0);
-  const int Ktot = Ktap * a.taps;
-  p.taps = a.taps;
+  const int Ktot = Ktap * ntaps;
+  p.taps = ntaps;
   p.kb_src1 = (a.K1 + BK - 1) / BK;
   p.kb_per_tap = p.kb_src1 + (two ? a.K2 / BK : 0);
-  p.num_kb = p.kb_per_tap * a.taps;
+  p.num_kb = p.kb_per_tap * ntaps;
   p.M = a.M;
   p.N = a.N;
   p.bias = a.bias;
@@ -534,13 +573,15 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   if (a.taps != 1) {
     VS_REQUIRE(a.nimg > 0 && a.H > 0 && a.W > 0 && a.M == a.nimg * a.H * a.W, "gemm_tc: bad conv geometry");
     p.a_rank = 4;
-    // 3x3: taps (-1..1)^2.  2x2 (one output parity (py, px) of nearest-2x + 3x3, see pack_conv_subpixel): taps
-    // {py - 1, py} x {px - 1, px}, output pixel (2 y + py, 2 x + px) of the 2H x 2W image.
+    // 3x3: taps (-1..1)^2.  Sub-pixel (one output parity (py, px) of nearest up-sampling + 3x3, see pack_conv_subpixel):
+    // taps {py - 1, py} x {px - 1, px}, output pixel (2 y + py, 2 x + px) of the OH x OW image; on an odd axis parity 0
+    // has the taps {-1, 0, 0'} with 0' read through the shifted view (tmS).
     if (a.taps == 9) { p.tap_x0 = p.tap_y0 = -1; p.tap_w = 3; p.osy = p.osx = 1; p.ooy = p.oox = 0; p.OH = a.H; p.OW = a.W; }
     else {
       VS_REQUIRE((a.sub_py | 1) == 1 && (a.sub_px | 1) == 1, "gemm_tc: sub-pixel parity must be 0 or 1");
-      p.tap_y0 = a.sub_py - 1; p.tap_x0 = a.sub_px - 1; p.tap_w = 2;
-      p.osy = p.osx = 2; p.ooy = a.sub_py; p.oox = a.sub_px; p.OH = 2 * a.H; p.OW = 2 * a.W;
+      p.tap_y0 = a.sub_py - 1; p.tap_x0 = a.sub_px - 1; p.tap_w = sub_tx;
+      ps.sub_short = (sub_ty == 3 ? 1 : 0) | (sub_tx == 3 ? 2 : 0);
+      p.osy = p.osx = 2; p.ooy = a.sub_py; p.oox = a.sub_px; p.OH = OH; p.OW = OW;
     }
     const ConvTile t = pick_conv_tile(a.nimg, a.H, a.W);
     p.nimg = a.nimg; p.H = a.H; p.W = a.W; p.TW = t.tw; p.TH = t.th; p.TN = t.tn;
@@ -554,6 +595,13 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
       const uint64_t dims[4] = {(uint64_t)a.K1, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.nimg};
       const uint64_t str[3] = {(uint64_t)a.lda1 * 2, (uint64_t)a.lda1 * 2 * a.W, (uint64_t)a.lda1 * 2 * a.W * a.H};
       if (make_tmap_f16(&p.tmA, a.A, 4, dims, str, box, 1)) return 3;
+      // shifted views for the third tap of an odd axis: element (x, y) of view k is element (x - [k != 0], y - [k != 1])
+      // of A; the kernel reads them at coordinates >= 1 only, so no address before A is touched
+      const long long shift[3] = {(long long)a.W * a.lda1, (long long)a.lda1, (long long)(a.W + 1) * a.lda1};
+      for (int k = 0; k < 3; ++k) {
+        const bool used = k == 2 ? ps.sub_short == 3 : ((ps.sub_short >> k) & 1) != 0;
+        if (used && make_tmap_f16(&ps.tmS[k], a.A - shift[k], 4, dims, str, box, 1)) return 3;
+      }
     }
     if (two) {
       const uint64_t dims[4] = {(uint64_t)a.K2, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.nimg};
@@ -607,12 +655,48 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
     if (p.ln_stats || p.ln_parts) return launch<256, EPI_F_GEGLU | EPI_F_LN>(st, p);
     return launch<256, EPI_F_GEGLU>(st, p);
   }
+  if (sub && ((OH | OW) & 1)) {
+    VS_REQUIRE(a.residual == nullptr && a.rowvec == nullptr && p.staged, "gemm_tc: an odd-sized sub-pixel conv takes a bias only");
+    switch (bn) {
+      case 64: return launch<64, 0, GemmParamsSub>(st, ps);
+      case 128: return launch<128, 0, GemmParamsSub>(st, ps);
+      case 256: return launch<256, 0, GemmParamsSub>(st, ps);
+      default: return launch<160, 0, GemmParamsSub>(st, ps);
+    }
+  }
   switch (bn) {
     case 64: return launch_linear<64>(st, p);
     case 128: return launch_linear<128>(st, p);
     case 256: return launch_linear<256>(st, p);
     default: return launch_linear<160>(st, p);
   }
+}
+
+// Panel of output parity (py, px) inside the up-sampler weights (see pack_conv_subpixel): the 3x3 panel itself when both
+// target axes are odd at parity (0, 0), else one of the panels of `wsub`.
+static const __half* subpixel_panel(const __half* w3x3, const __half* wsub, int cout, int cin, int py, int px, bool odd_y,
+                                    bool odd_x) {
+  const bool ty3 = py == 0 && odd_y, tx3 = px == 0 && odd_x;
+  const size_t tap = (size_t)cout * cin;
+  if (ty3 && tx3) return w3x3;
+  if (ty3) return wsub + (16 + 6 * px) * tap;
+  if (tx3) return wsub + (28 + 6 * py) * tap;
+  return wsub + (size_t)(2 * py + px) * 4 * tap;
+}
+
+int upsample_conv3x3(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, const __half* w3x3, const __half* wsub,
+                     const float* bias, int cout, int OH, int OW, __half* out) {
+  VS_REQUIRE((OH == 2 * H || OH == 2 * H - 1) && (OW == 2 * W || OW == 2 * W - 1),
+             "upsample_conv3x3: output %dx%d is not 2x (or 2x - 1) of the %dx%d input", OH, OW, H, W);
+  VS_REQUIRE(w3x3 != nullptr || ((OH & 1) == 0 && (OW & 1) == 0), "upsample_conv3x3: odd output sizes need the 3x3 panel");
+  for (int par = 0; par < 4; ++par) {
+    GemmArgs g;
+    g.A = x; g.K1 = C; g.lda1 = C; g.Bw = subpixel_panel(w3x3, wsub, cout, C, par >> 1, par & 1, OH & 1, OW & 1); g.taps = 4;
+    g.sub_py = par >> 1; g.sub_px = par & 1; g.OH = OH; g.OW = OW; g.nimg = nimg; g.H = H; g.W = W; g.M = nimg * H * W;
+    g.N = cout; g.bias = bias; g.out = out; g.ldc = cout;
+    if (int e = gemm_tc(st, g)) return e;
+  }
+  return 0;
 }
 
 }  // namespace vs

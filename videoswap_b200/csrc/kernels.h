@@ -20,9 +20,9 @@ struct GemmArgs {
   const __half* A2 = nullptr; int K2 = 0;  int lda2 = 0;
   const __half* Bw = nullptr;                 // [N, taps*(K1+K2)] fp16, K contiguous
   int M = 0, N = 0;
-  int taps = 1;                               // 1, 9 (3x3, pad 1) or 4 (2x2 sub-pixel phase of nearest-2x + 3x3)
-  int sub_py = 0, sub_px = 0;                 // taps == 4: output parity; writes pixel (2y+py, 2x+px) of the 2H x 2W output
-  int nimg = 0, H = 0, W = 0;                 // conv geometry (taps == 9)
+  int taps = 1;                               // 1, 9 (3x3, pad 1) or 4 (sub-pixel phase of nearest up-sampling + 3x3)
+  int sub_py = 0, sub_px = 0;                 // taps == 4: output parity; writes pixel (2y+py, 2x+px) of the OH x OW output
+  int nimg = 0, H = 0, W = 0;                 // conv geometry (taps == 9 / 4)
   const float* bias = nullptr;                // [N] fp32
   const float* rowvec = nullptr;              // [M / pix_per_batch, ldrv] fp32 (time-embedding add)
   int ldrv = 0;                               // row stride of rowvec (0 = N)
@@ -41,6 +41,9 @@ struct GemmArgs {
   __half* out = nullptr; int ldc = 0;
   int mode = EPI_LINEAR;
   int force_bn = 0;                           // 0 = auto
+  // taps == 4: output extent, 2H or 2H - 1 rows and 2W or 2W - 1 columns (0 = 2H / 2W).  Along an odd axis parity 0 has
+  // 3 taps, so Bw holds 2x3, 3x2 or 3x3 taps (the panels pack_conv_subpixel / pack_conv3x3 make, see upsample_conv3x3).
+  int OH = 0, OW = 0;
 };
 int gemm_tc(cudaStream_t st, const GemmArgs& a);
 int gemm_n_tiles(const GemmArgs& a);         // column tiles gemm_tc will use (taps == 1)
@@ -98,7 +101,8 @@ int timestep_embedding(cudaStream_t st, const float* t, int B, int dim, float* o
 int conv_in_3x3(cudaStream_t st, const __half* x, int nimg, int H, int W, int cin, const __half* w, const float* bias,
                 int cout, __half* out, __half* scratch = nullptr);   // conv_in (tiny Cin): with `scratch` (>= (nimg*H*W +
                 // cout) * 64 halves, cin == 4) patch rows + tensor-core GEMM, else a direct CUDA-core kernel
-int upsample_nearest2x(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out);
+// nearest up-sampling by 2 to an OH x OW output (OH in {2H - 1, 2H}, OW in {2W - 1, 2W}): out[y, x] = in[y / 2, x / 2]
+int upsample_nearest2x(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out, int OH = 0, int OW = 0);
 int im2col_s2(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out);  // [nimg*Ho*Wo, 9*C]
 int add_inplace(cudaStream_t st, __half* x, const __half* r, size_t n, float scale);   // x += scale * r
 int ncfhw_to_nhwc(cudaStream_t st, const void* src, int src_is_f32, int B, int C, int F, int H, int W, __half* dst);
@@ -138,7 +142,16 @@ int pack_conv3x3(cudaStream_t st, const __half* w, int cout, int cin, __half* ou
 // (py = 1), so the 3 row taps collapse to 2 with weights {w[-1], w[0]+w[1]} / {w[-1]+w[0], w[1]}; same along x.
 // out: [4 parities (py*2+px)][co][2x2 taps][ci] fp16 (weights summed in fp32, rounded once).  2.25x fewer FLOPs and no
 // materialised up-sampled tensor.
-int pack_conv_subpixel(cudaStream_t st, const __half* w, int cout, int cin, __half* out);
+// With odd_panels, 4 more panels follow for targets of odd size 2n - 1 (F.interpolate(size=...) of the reference's
+// forward_upsample_size path): there row 2n - 1 of the up-sampled image is padding, so parity 0 keeps the taps
+// {w[-1], w[0], w[1]} apart (the third one reads a shifted view, see gemm.cu): [co][3x2 taps][ci] for (py, px) = (0, 0),
+// (0, 1) with an odd height, then [co][2x3 taps][ci] for (0, 0), (1, 0) with an odd width (24 taps; 40 in all).  Parity
+// (0, 0) with both axes odd is the plain 3x3 panel (pack_conv3x3).
+int pack_conv_subpixel(cudaStream_t st, const __half* w, int cout, int cin, __half* out, bool odd_panels = false);
+// Upsample3D: nearest up-sampling of NHWC x [nimg, H, W, C] to OH x OW, then the 3x3 conv, as 4 sub-pixel launches.
+// w3x3: pack_conv3x3 panel (needed only for odd OH / OW); wsub: pack_conv_subpixel panels (with odd_panels for odd sizes).
+int upsample_conv3x3(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, const __half* w3x3, const __half* wsub,
+                     const float* bias, int cout, int OH, int OW, __half* out);
 int pack_geglu(cudaStream_t st, const __half* w, const __half* b, int hidden, int K, int granule, __half* wout,
                float* bout);   // rows interleaved value/gate in `granule` blocks; w or b may be null (pack one only)
 int f16_to_f32(cudaStream_t st, const __half* x, size_t n, float* out);

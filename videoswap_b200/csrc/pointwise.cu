@@ -124,13 +124,15 @@ __global__ void conv_in_pack_kernel(const __half* __restrict__ w, int cout, __ha
 }
 
 // ---------------------------------------------------------------------------------------------- data movement
-__global__ void upsample2x_kernel(const uint4* __restrict__ x, int nimg, int H, int W, int CV, uint4* __restrict__ out) {
-  const long long total = (long long)nimg * 4 * H * W * CV;
+// nearest up-sampling to OH x OW with OH in {2H - 1, 2H}: torch's source row floor(yo * H / OH) is yo / 2 for both
+__global__ void upsample2x_kernel(const uint4* __restrict__ x, int nimg, int H, int W, int CV, int OH, int OW,
+                                  uint4* __restrict__ out) {
+  const long long total = (long long)nimg * OH * OW * CV;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int cv = i % CV;
     const long long pix = i / CV;
-    const int xo = pix % (2 * W), yo = (pix / (2 * W)) % (2 * H);
-    const long long img = pix / (4LL * W * H);
+    const int xo = pix % OW, yo = (pix / OW) % OH;
+    const long long img = pix / ((long long)OW * OH);
     out[i] = x[((img * H + yo / 2) * W + xo / 2) * CV + cv];
   }
 }
@@ -385,6 +387,32 @@ __global__ void pack_conv_subpixel_kernel(const __half* __restrict__ w, int cout
     out[i] = __float2half_rn(acc);
   }
 }
+// The 4 panels of odd target sizes (pack_conv_subpixel with odd_panels): along the odd axis parity 0 has the three
+// unsummed taps {0}, {1}, {2}; the other axis collapses as above.  Panels: (py, px) = (0, 0), (0, 1) with 3 row taps,
+// then (0, 0), (1, 0) with 3 column taps; 6 taps each.
+__global__ void pack_conv_subpixel_odd_kernel(const __half* __restrict__ w, int cout, int cin, __half* __restrict__ out) {
+  const long long per = (long long)cout * 6 * cin, total = 4 * per;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int ci = i % cin, tap = (i / cin) % 6;
+    const long long co = (i / (6LL * cin)) % cout;
+    const int panel = i / per;
+    const bool odd_rows = panel < 2;
+    const int py = odd_rows ? 0 : panel - 2, px = odd_rows ? panel : 0;
+    const int ty = odd_rows ? tap >> 1 : tap / 3, tx = odd_rows ? tap & 1 : tap % 3;   // slot along y / x
+    auto range = [](int par, bool three, int t, int& a, int& b) {
+      if (three) { a = b = t; return; }
+      a = (par == 0) ? (t == 0 ? 0 : 1) : (t == 0 ? 0 : 2);
+      b = (par == 0) ? (t == 0 ? 0 : 2) : (t == 0 ? 1 : 2);
+    };
+    int r0, r1, c0, c1;
+    range(py, odd_rows, ty, r0, r1);
+    range(px, !odd_rows, tx, c0, c1);
+    float acc = 0.f;
+    for (int r = r0; r <= r1; ++r)
+      for (int c = c0; c <= c1; ++c) acc += __half2float(w[(co * cin + ci) * 9 + r * 3 + c]);
+    out[i] = __float2half_rn(acc);
+  }
+}
 __global__ void pack_geglu_kernel(const __half* __restrict__ w, const __half* __restrict__ b, int hidden, int K,
                                   int gran, __half* __restrict__ wout, float* __restrict__ bout) {
   const long long total = (long long)2 * hidden * K;
@@ -495,10 +523,14 @@ int conv_in_3x3(cudaStream_t st, const __half* x, int nimg, int H, int W, int ci
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
-int upsample_nearest2x(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out) {
+int upsample_nearest2x(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out, int OH, int OW) {
   VS_REQUIRE(C % 8 == 0, "upsample: C %% 8 != 0");
-  upsample2x_kernel<<<capped((size_t)nimg * 4 * H * W * (C / 8)), TPB, 0, st>>>(
-      reinterpret_cast<const uint4*>(x), nimg, H, W, C / 8, reinterpret_cast<uint4*>(out));
+  if (OH <= 0) OH = 2 * H;
+  if (OW <= 0) OW = 2 * W;
+  VS_REQUIRE((OH == 2 * H || OH == 2 * H - 1) && (OW == 2 * W || OW == 2 * W - 1),
+             "upsample: output %dx%d is not 2x (or 2x - 1) of the %dx%d input", OH, OW, H, W);
+  upsample2x_kernel<<<capped((size_t)nimg * OH * OW * (C / 8)), TPB, 0, st>>>(
+      reinterpret_cast<const uint4*>(x), nimg, H, W, C / 8, OH, OW, reinterpret_cast<uint4*>(out));
   count_launch(1);
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -591,9 +623,13 @@ int pack_conv3x3(cudaStream_t st, const __half* w, int cout, int cin, __half* ou
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
-int pack_conv_subpixel(cudaStream_t st, const __half* w, int cout, int cin, __half* out) {
+int pack_conv_subpixel(cudaStream_t st, const __half* w, int cout, int cin, __half* out, bool odd_panels) {
   pack_conv_subpixel_kernel<<<capped((size_t)cout * 16 * cin), TPB, 0, st>>>(w, cout, cin, out);
   count_launch(1);
+  if (odd_panels) {
+    pack_conv_subpixel_odd_kernel<<<capped((size_t)cout * 24 * cin), TPB, 0, st>>>(w, cout, cin, out + (size_t)cout * 16 * cin);
+    count_launch(1);
+  }
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -28,7 +28,7 @@ struct Loader {
 };
 
 struct Lin { __half* w = nullptr; float* b = nullptr; int N = 0, K = 0; };
-struct Conv3 { __half* w = nullptr; float* b = nullptr; int co = 0, ci = 0; __half* wsub = nullptr; };   // wsub: 4 sub-pixel panels
+struct Conv3 { __half* w = nullptr; float* b = nullptr; int co = 0, ci = 0; __half* wsub = nullptr; };   // wsub: sub-pixel panels
 struct Norm { float* g = nullptr; float* b = nullptr; int C = 0; };
 // A linear layer with the LayerNorm in front of it folded in (kernels.h ln_fold): gamma-scaled weights, row sums, offsets
 struct LnLin { __half* wf = nullptr; float* u = nullptr; float* c = nullptr; float* cpe = nullptr; };
@@ -312,9 +312,9 @@ extern "C" int vs_unet_create(const vs_unet_config* cfg, vs_unet** out) {
     }
     if (i < 3) {
       b.has_sampler = true;
-      Conv3& c = b.sampler;           // [co, 9, ci] followed by 4 x [co, 4, ci]
+      Conv3& c = b.sampler;           // [co, 9, ci] followed by the 40 taps of pack_conv_subpixel (even + odd target sizes)
       c.co = oc; c.ci = oc;
-      c.w = h->alloc<__half>((size_t)oc * 9 * oc + (size_t)16 * oc * oc);
+      c.w = h->alloc<__half>((size_t)oc * 9 * oc + (size_t)40 * oc * oc);
       c.wsub = c.w + (size_t)oc * 9 * oc;
       h->reg(p + ".upsamplers.0.conv.weight", LK_CONV_UP, c.w, (int64_t)oc * oc * 9, oc, oc);
       c.b = h->f32(p + ".upsamplers.0.conv.bias", oc);
@@ -359,9 +359,9 @@ extern "C" int vs_unet_load_weights(vs_unet* h, void* stream, int n, const char*
         break;
       case LK_TO_F32: e = f16_to_f32(st, src, (size_t)L.numel, (float*)L.dst); break;
       case LK_CONV3: e = pack_conv3x3(st, src, L.a, L.b, (__half*)L.dst); break;
-      case LK_CONV_UP:                  // up-sampler conv: the plain 3x3 panel (A/B path) and the four 2x2 sub-pixel panels
-        e = pack_conv3x3(st, src, L.a, L.b, (__half*)L.dst);
-        if (!e) e = pack_conv_subpixel(st, src, L.a, L.b, (__half*)L.dst + (size_t)L.a * 9 * L.b);
+      case LK_CONV_UP:                  // up-sampler conv: the plain 3x3 panel (A/B path, and parity (0, 0) of an odd-sized
+        e = pack_conv3x3(st, src, L.a, L.b, (__half*)L.dst);             // target) and the sub-pixel panels
+        if (!e) e = pack_conv_subpixel(st, src, L.a, L.b, (__half*)L.dst + (size_t)L.a * 9 * L.b, true);
         break;
       case LK_GEGLU_W: e = pack_geglu(st, src, nullptr, L.a, L.b, kGegluGranule, (__half*)L.dst, nullptr); break;
       case LK_GEGLU_B: e = pack_geglu(st, nullptr, src, L.a, 1, kGegluGranule, nullptr, (float*)L.dst); break;
@@ -748,6 +748,17 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
   VS_REQUIRE(ehs_tokens >= 1 && ehs_tokens <= 128, "vs_unet_forward: ehs_tokens out of range");
   VS_REQUIRE(h->cfg.in_channels <= 8 && h->cfg.out_channels <= 8, "in/out channels > 8 unsupported");
   VS_REQUIRE(h->fnshards == 1 || B == 1, "frame-sharded forward: one batch element per rank (got B = %d)", B);
+  // Level sizes follow the stride-2 convs of the down path: H_{l+1} = ceil(H_l / 2).  Each up-sampler targets the size of
+  // the skip it feeds (the reference's forward_upsample_size path), so any H, W >= 1 runs; all checks happen here, before
+  // the first launch.
+  int lvH[4], lvW[4];
+  lvH[0] = H; lvW[0] = W;
+  for (int l = 1; l < 4; ++l) { lvH[l] = (lvH[l - 1] + 1) / 2; lvW[l] = (lvW[l - 1] + 1) / 2; }
+  if (h->fnshards > 1) {
+    for (int l = 0; l < 4; ++l)
+      VS_REQUIRE((lvH[l] * lvW[l]) % h->fnshards == 0, "frame sharding needs h*w of every level divisible by the %d shards "
+                 "(level %d is %dx%d)", h->fnshards, l, lvH[l], lvW[l]);
+  }
   cudaStream_t st = (cudaStream_t)stream;
   RUN(ensure_workspace(h, B, F, H, W));
   if (h->folds_dirty) {
@@ -859,27 +870,24 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
       cur = o;
     }
     if (blk.has_sampler) {
-      // Upsample3D: nearest [1,2,2] then 3x3 conv (resnet.py:54,67) = four 2x2 sub-pixel convs on the low-resolution input
-      // (2.25x fewer FLOPs, the up-sampled tensor is never written); "subpixel" = 0 keeps the materialising path (A/B)
+      // Upsample3D: nearest up-sampling to the size of the next skip (2x, or 2x - 1 where that level was odd; resnet.py:
+      // 51-56, unet.py:454-457) then 3x3 conv = four sub-pixel convs on the low-resolution input (2.25x fewer FLOPs, the
+      // up-sampled tensor is never written); "subpixel" = 0 keeps the materialising path (A/B)
       __half* o = (cur == h->P0) ? h->P1 : h->P0;
+      const int OH = lvH[2 - i], OW = lvW[2 - i];
       if (get_option("subpixel") != 0) {
-        for (int par = 0; par < 4; ++par) {
-          GemmArgs g;
-          g.A = cur; g.K1 = curC; g.lda1 = curC; g.Bw = blk.sampler.wsub + (size_t)par * blk.sampler.co * 4 * curC; g.taps = 4;
-          g.sub_py = par >> 1; g.sub_px = par & 1; g.nimg = c.NI; g.H = c.H; g.W = c.W; g.M = c.NI * c.H * c.W; g.N = blk.sampler.co;
-          g.bias = blk.sampler.b; g.out = o; g.ldc = blk.sampler.co;
-          RUN(gemm_tc(st, g));
-        }
-        c.H *= 2; c.W *= 2;
+        RUN(upsample_conv3x3(st, cur, c.NI, c.H, c.W, curC, blk.sampler.w, blk.sampler.wsub, blk.sampler.b, blk.sampler.co,
+                             OH, OW, o));
+        c.H = OH; c.W = OW;
       } else {
-        RUN(upsample_nearest2x(st, cur, c.NI, c.H, c.W, curC, h->SCR));
-        c.H *= 2; c.W *= 2;
+        RUN(upsample_nearest2x(st, cur, c.NI, c.H, c.W, curC, h->SCR, OH, OW));
+        c.H = OH; c.W = OW;
         RUN(conv(c, h->SCR, curC, blk.sampler, nullptr, nullptr, o));
       }
       cur = o;
     }
   }
-  VS_REQUIRE(c.H == H && c.W == W, "input H/W (%d,%d) must be multiples of 8 (the reference's forward_upsample_size path is not implemented)", H, W);
+  VS_REQUIRE(c.H == H && c.W == W, "internal: the up path ended at %dx%d, not at the input's %dx%d", c.H, c.W, H, W);
   // ---- out: GroupNorm(5-D) + SiLU + conv_out
   NEXT_SUMS(osums);
   RUN(groupnorm_stats(st, cur, curC, nullptr, 0, c.NI, H * W, F, cf.norm_num_groups, osums, false));

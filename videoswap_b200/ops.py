@@ -156,6 +156,31 @@ def upsample_conv3x3(x, w, bias=None):
     return out
 
 
+def upsample_conv3x3_sized(x, w, bias, OH, OW, out=None):
+    """nearest up-sampling to OH x OW (2H or 2H - 1 rows, 2W or 2W - 1 columns) + conv3x3 (pad 1), as the UNet's up path
+    runs it: x [N, H, W, C], w [Co, C, 3, 3] (unpacked) -> [N, OH, OW, Co].  `out` may be any contiguous fp16 buffer of at
+    least N * OH * OW * Co elements; the result is its first N * OH * OW * Co elements."""
+    _chk16(x, w, out)
+    _chk32(bias)
+    n, H, W, Ci = x.shape
+    co = w.shape[0]
+    panels = torch.empty((49 * co * Ci,), dtype=torch.float16, device=x.device)
+    if out is None:
+        out = torch.empty((n, OH, OW, co), dtype=torch.float16, device=x.device)
+    assert out.is_contiguous() and out.numel() >= n * OH * OW * co
+    _lib.call("vs_upsample_conv3x3_sized", _stream(), _p(x), n, H, W, Ci, _p(w), co, _p(bias), OH, OW, _p(panels), _p(out))
+    return out
+
+
+def upsample_nearest(x, OH, OW):
+    """x [N, H, W, C] -> [N, OH, OW, C], out[y, x] = in[y // 2, x // 2] (OH in {2H - 1, 2H}, OW in {2W - 1, 2W})."""
+    _chk16(x)
+    n, H, W, Cc = x.shape
+    out = torch.empty((n, OH, OW, Cc), dtype=torch.float16, device=x.device)
+    _lib.call("vs_upsample_nearest", _stream(), _p(x), n, H, W, Cc, OH, OW, _p(out))
+    return out
+
+
 def groupnorm(x1, gamma, beta, groups, eps, imgs_per_set=1, silu=False, x2=None):
     """x1 [N, H, W, C1] (+ x2) -> normalised [N, H, W, C1+C2]; statistics over imgs_per_set images x (C/groups)."""
     _chk16(x1, x2)

@@ -452,6 +452,24 @@ class AnimateDiffUNet3DModel(nn.Module):
                     idx += 1
         return controller
 
+    def level_sizes(self, H: int, W: int):
+        """(H_l, W_l) of the four levels: the stride-2 convs of the down path give H_{l+1} = ceil(H_l / 2)."""
+        sizes = [(H, W)]
+        for _ in range(3):
+            h, w = sizes[-1]
+            sizes.append(((h + 1) // 2, (w + 1) // 2))
+        return sizes
+
+    def _check_residuals(self, residuals, n, H, W):
+        """The library reads residual l as [(B F), C_l, H_l, W_l]: anything else is refused before any launch."""
+        if len(residuals) > 4:
+            raise ValueError(f"down_block_additional_residuals: at most 4 tensors, got {len(residuals)}")
+        for l, (r, (h, w)) in enumerate(zip(residuals, self.level_sizes(H, W))):
+            want = (n, self.cfg.block_out_channels[l], h, w)
+            if tuple(r.shape) != want:
+                raise ValueError(f"down_block_additional_residuals[{l}] has shape {tuple(r.shape)}; the UNet reads "
+                                 f"{list(want)} ([(B F), C_l, H_l, W_l] with H_l = ceil(H_(l-1) / 2)) at latent {H}x{W}")
+
     def __del__(self):
         try:
             if self._handle is not None:
@@ -474,10 +492,13 @@ class AnimateDiffUNet3DModel(nn.Module):
         B, Cin, F, H, W = sample.shape
         if Cin != self.cfg.in_channels:
             raise ValueError(f"sample has {Cin} channels, expected {self.cfg.in_channels}")
-        if H % 8 or W % 8:
-            raise NotImplementedError("latent H and W must be multiples of 8")
         dev = sample.device
         controller = self._check_processors()
+        if controller is not None and (H % 8 or W % 8):
+            raise NotImplementedError("attention controllers need latent H and W to be multiples of 8 (their latent blend "
+                                      "rebuilds each map's height and width from its token count and the aspect ratio)")
+        if down_block_additional_residuals is not None:
+            self._check_residuals(down_block_additional_residuals, B * F, H, W)
         with torch.cuda.device(dev):
             self._sync_weights(dev)
             io_f32 = sample.dtype == torch.float32
