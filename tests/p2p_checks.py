@@ -9,6 +9,7 @@ import torch
 
 from oracle import make_golden_p2p as G
 from oracle import unet3d_oracle as O
+from tests import attention_probes as A
 from tests import unet_checks as U
 from videoswap_b200 import ops, p2p
 
@@ -17,7 +18,9 @@ DEV = "cuda"
 
 
 def explicit_attention_check(B=3, N=256, NK=None, C=1280, kv_div=1, seed=170):
-    """probs = softmax(q k^T / sqrt(d)) to HBM, then O = P V, vs fp32 torch (d = C / 8)."""
+    """probs = softmax(q k^T / sqrt(d)) to HBM, then O = P V (d = C / 8).  The probabilities element by element against
+    the fp64 softmax and O against fp64 P V of the probabilities the kernel wrote, both with the bounds of
+    tests/attention_probes.py ("probs" / "out": err = the worst err / bound); O also against fp32 torch."""
     g = torch.Generator().manual_seed(seed)
     NK = N if NK is None else NK
     q = torch.randn((B, N, C), generator=g).half().to(DEV)
@@ -32,7 +35,12 @@ def explicit_attention_check(B=3, N=256, NK=None, C=1280, kv_div=1, seed=170):
     vh = v.float().repeat_interleave(kv_div, 0).reshape(B, NK, 8, d).transpose(1, 2)
     pr = (qh @ kh.transpose(-1, -2) * d ** -0.5).softmax(-1)
     ref = (pr @ vh).transpose(1, 2).reshape(B, N, C)
-    return {"probs_err": (probs.float() - pr).abs().max().item(), "row_sum_err": (probs.float().sum(-1) - 1).abs().max().item(),
+    vd = v.double().repeat_interleave(kv_div, 0).reshape(B, NK, 8, d).transpose(1, 2)
+    pv = (probs.double() @ vd).transpose(1, 2).reshape(B, N, C)
+    mag = (probs.double() @ vd.abs()).transpose(1, 2).reshape(B, N, C)
+    return {"probs": A.compare(probs, A.ref_probs(q, k, 8, kv_div), rel=A.PROBS_REL),
+            "out": A.compare(out, pv, rel=A.PV_REL, extra=A.pv_extra(NK) * mag),
+            "row_sum_err": (probs.float().sum(-1) - 1).abs().max().item(),
             "out_err": (out.float() - ref).abs().max().item(), "out_ref": ref.abs().max().item()}
 
 
