@@ -297,18 +297,20 @@ __device__ __forceinline__ float gelu_erf_fast(float x) {
   return 0.5f * x * (1.f + erf_s);
 }
 // erf-GELU in logistic form, x * Phi(x) = x / (1 + 2^(-x q(x^2))): q is a cubic in x^2 fitted (minimax, |x| <= 5, argument
-// clamped beyond) to log2(Phi / (1 - Phi)) / x.  |error| <= 1.2e-5 absolute over all x -- below the fp16 rounding of the
-// result for |gelu| > 0.02 -- at 2 MUFU + 9 FP32 instructions (gelu_erf_fast: 2 MUFU + ~16); used by the GEGLU GEMM
-// epilogue, whose instruction count bounds the K = 320 feed-forward GEMM.
+// clamped beyond) to log2(Phi / (1 - Phi)) / x.  |error| <= 1.2e-5 + 2^-20 |x| over all x -- below the fp16 rounding of
+// the result for |gelu| > 0.02 -- at 2 MUFU + 9 FP32 instructions (gelu_erf_fast: 2 MUFU + ~16); used by the GEGLU GEMM
+// epilogue, whose instruction count bounds the K = 320 feed-forward GEMM.  The numerator is clamped at -5 too: beyond
+// it 1 + e is ~1.5e6, so an unclamped x would return x / 1.5e6 (-0.04 at x = -65504) instead of ~0.
 __device__ __forceinline__ float gelu_sig(float x) {
-  const float xc = fminf(fmaxf(x, -5.f), 5.f);
+  const float xn = fmaxf(x, -5.f);
+  const float xc = fminf(xn, 5.f);
   const float u = xc * xc;
   float q = fmaf(u, 2.47135360e-05f, 7.37690930e-04f);      // coefficients negated: t = -x q(x^2)
   q = fmaf(q, u, -1.05988323e-01f);
   q = fmaf(q, u, -2.30164247e+00f);
   float e;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(xc * q));
-  return __fdividef(x, 1.f + e);
+  return __fdividef(xn, 1.f + e);
 }
 #endif  // __CUDACC__
 

@@ -34,9 +34,25 @@ __device__ __forceinline__ uint4 gn_load(const GnParams& p, long long pix, int c
   return *reinterpret_cast<const uint4*>(p.x2 + pix * p.c2 + (c - p.c1));
 }
 
-// V2: eight per-position (sum, sum of squares) accumulators without predicates (3 instructions per element instead of ~10
-// for the per-element group select of V1, whose issue slots -- 64 % active -- bounded the pass); the group split is applied
-// once per thread at the end.
+__device__ __forceinline__ float gn_load1(const GnParams& p, long long pix, int c) {
+  return __half2float(c < p.c1 ? p.x1[pix * p.c1 + c] : p.x2[pix * p.c2 + (c - p.c1)]);
+}
+
+// Shifted sums.  Summing x and x^2 directly loses the variance to cancellation once the mean is large against the spread
+// (E[x^2] - mean^2 with fp32 sums of ~|mean|^2-sized terms).  Every block (every CTA of a cluster) therefore sums
+// d = x - k_g with one shift per group, k_g = the group's first channel at the block's first pixel, and converts its
+// partial back to plain sums before adding it to the global (or cluster) total: S = S' + m k, Q = Q' + k (2 S' + m k)
+// over the block's m elements of the group.  The long per-thread and shared-atomic runs then add spread-sized terms,
+// and the buffer still holds plain (sum, sum of squares), so frame shards that all-reduce it need no common shift.
+__device__ __forceinline__ void gn_unshift(float& s, float& q, float k, float m) {
+  const float mk = m * k;
+  q = fmaf(k, s + s + mk, q);
+  s += mk;
+}
+
+// V2: eight per-position (sum, sum of squares) accumulators without predicates (4 instructions per element instead of
+// ~11 for the per-element group select of V1, whose issue slots -- 64 % active -- bounded the pass); the group split is
+// applied once per thread at the end.
 template <bool V2>
 __global__ void gn_stats_kernel(const GnParams p) {
   extern __shared__ float sh[];   // [groups][2]
@@ -53,17 +69,22 @@ __global__ void gn_stats_kernel(const GnParams p) {
   const long long p0 = (long long)blockIdx.x * p.pix_per_block;
   const long long p1 = min(p0 + p.pix_per_block, p.pix_per_set);
   const long long base = (long long)set * p.pix_per_set;
+  const float ka = gn_load1(p, base + p0, ga * p.cpg), kb = gn_load1(p, base + p0, gb * p.cpg);   // the block's shifts
+  float ks[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) ks[j] = j < split ? ka : kb;
   auto accum = [&](const uint4& v) {
     const __half2* h = reinterpret_cast<const __half2*>(&v);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 f = __half22float2(h[j]);
+      const float dx = f.x - ks[2 * j], dy = f.y - ks[2 * j + 1];
       if (V2) {
-        ps[2 * j] += f.x; pq[2 * j] = fmaf(f.x, f.x, pq[2 * j]);
-        ps[2 * j + 1] += f.y; pq[2 * j + 1] = fmaf(f.y, f.y, pq[2 * j + 1]);
+        ps[2 * j] += dx; pq[2 * j] = fmaf(dx, dx, pq[2 * j]);
+        ps[2 * j + 1] += dy; pq[2 * j + 1] = fmaf(dy, dy, pq[2 * j + 1]);
       } else {
-        if (2 * j < split) { sa += f.x; qa += f.x * f.x; } else { sb += f.x; qb += f.x * f.x; }
-        if (2 * j + 1 < split) { sa += f.y; qa += f.y * f.y; } else { sb += f.y; qb += f.y * f.y; }
+        if (2 * j < split) { sa += dx; qa += dx * dx; } else { sb += dx; qb += dx * dx; }
+        if (2 * j + 1 < split) { sa += dy; qa += dy * dy; } else { sb += dy; qb += dy * dy; }
       }
     }
   };
@@ -88,7 +109,13 @@ __global__ void gn_stats_kernel(const GnParams p) {
     atomicAdd(&sh[gb * 2 + 1], qb);
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < p.groups * 2; i += blockDim.x) atomicAdd(&p.sums[(long long)set * p.groups * 2 + i], sh[i]);
+  const float m = (float)((p1 - p0) * p.cpg);                      // elements of a group in this block
+  for (int g = threadIdx.x; g < p.groups; g += blockDim.x) {
+    float s = sh[2 * g], q = sh[2 * g + 1];
+    gn_unshift(s, q, gn_load1(p, base + p0, g * p.cpg), m);
+    atomicAdd(&p.sums[((long long)set * p.groups + g) * 2], s);
+    atomicAdd(&p.sums[((long long)set * p.groups + g) * 2 + 1], q);
+  }
 }
 
 __global__ void gn_apply_kernel(const GnParams p) {
@@ -158,15 +185,23 @@ __global__ void __launch_bounds__(kGnFusedThreads, 1) gn_frame_fused_kernel(cons
   pdl_wait();
   const int ga = (cv * 8) / p.cpg, gb = (cv * 8 + 7) / p.cpg;
   const int split = (ga == gb) ? 8 : (gb * p.cpg - cv * 8);
-  const uint4* src = reinterpret_cast<const uint4*>(p.x1) + ((long long)img * p.hw + (long long)rank * ppc) * p.CV + cv;
+  const long long pix0 = (long long)img * p.hw + (long long)rank * ppc;   // this CTA's first pixel
+  const uint4* src = reinterpret_cast<const uint4*>(p.x1) + pix0 * p.CV + cv;
   float ps[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, pq[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float ks[8];                                                    // shifted sums (see gn_unshift), one shift per group
+  {
+    const float ka = gn_load1(p, pix0, ga * p.cpg), kb = gn_load1(p, pix0, gb * p.cpg);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) ks[j] = j < split ? ka : kb;
+  }
   auto accum = [&](const uint4& v) {
     const __half2* h = reinterpret_cast<const __half2*>(&v);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const float2 f = __half22float2(h[j]);
-      ps[2 * j] += f.x; pq[2 * j] = fmaf(f.x, f.x, pq[2 * j]);
-      ps[2 * j + 1] += f.y; pq[2 * j + 1] = fmaf(f.y, f.y, pq[2 * j + 1]);
+      const float dx = f.x - ks[2 * j], dy = f.y - ks[2 * j + 1];
+      ps[2 * j] += dx; pq[2 * j] = fmaf(dx, dx, pq[2 * j]);
+      ps[2 * j + 1] += dy; pq[2 * j + 1] = fmaf(dy, dy, pq[2 * j + 1]);
     }
   };
   int i = r;
@@ -192,6 +227,9 @@ __global__ void __launch_bounds__(kGnFusedThreads, 1) gn_frame_fused_kernel(cons
     atomicAdd(&part[gb * 2], sb);
     atomicAdd(&part[gb * 2 + 1], qb);
   }
+  __syncthreads();
+  if (threadIdx.x < p.groups) gn_unshift(part[2 * threadIdx.x], part[2 * threadIdx.x + 1], gn_load1(p, pix0, threadIdx.x * p.cpg),
+                                        (float)(ppc * p.cpg));
   __syncthreads();
   if (ncta > 1) cluster_sync_all();                               // every CTA's partial sums are complete
   if (threadIdx.x < 64) {
