@@ -241,8 +241,31 @@ int vs_upsample_nearest(void* stream, const void* d_x, int nimg, int H, int W, i
 int vs_conv3x3_s2(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w_packed, int Cout,
                   const float* d_bias, void* d_scratch, void* d_out);
 
+/* ---- VAE decoder (diffusers 0.19.3 AutoencoderKL.decode + VaeImageProcessor.postprocess; the reference's loop ends with
+ * them, pipeline_videoswap.py:603-610).  The decoder is a sequence of the GEMM / conv / GroupNorm entry points above and
+ * these five. */
+/* The four sub-pixel panels of vs_upsample_conv3x3 (d_out: 16 * cout * cin halves), packed once so that the four parity
+ * launches (vs_gemm_ex, taps 4, Bw = panel py * 2 + px) can run without re-packing. */
+int vs_pack_conv_subpixel(void* stream, const void* d_w, int cout, int cin, void* d_out);
+/* Single-head attention with d = 512 (the VAE mid block) as S = Q K^T -> P -> O = P V through vs_gemm_ex:
+ * vs_softmax_rows: d_s [rows, ld] fp16 in place, p = softmax(s * scale) over the first n columns with fp32 math; columns
+ * n .. ld - 1 are set to 0 and never read (ld % 8 == 0).
+ * vs_transpose_pad: d_dst [cols, rows_pad] = d_src [rows, cols]^T (fp16), columns rows .. rows_pad - 1 zero: V^T as the
+ * K-major B operand of O = P V with K = rows_pad. */
+int vs_softmax_rows(void* stream, void* d_s, int rows, int n, int ld, float scale);
+int vs_transpose_pad(void* stream, const void* d_src, int rows, int cols, int rows_pad, void* d_dst);
+/* Decoder entry: post_quant_conv(z / divisor) of NCHW latents d_z [nimg, 4, h, w] (fp16, or fp32 with z_is_f32) in fp32,
+ * to NHWC fp16 d_out [nimg, h, w, 4].  d_wb: fp32 weight [4][4] then bias [4]. */
+int vs_vae_latent_in(void* stream, const void* d_z, int z_is_f32, int nimg, int h, int w, float divisor, const float* d_wb,
+                     void* d_out);
+/* Decoder exit: channels 0..2 of NHWC fp16 d_x [nimg, H, W, channels] (channels % 8 == 0), y = clamp(x / 2 + 0.5, 0, 1):
+ * format 0 the sample x itself, fp16 NCHW [nimg, 3, H, W]; 1 ("pt") y fp32 NCHW; 2 ("np") y fp32 NHWC [nimg, H, W, 3];
+ * 3 ("pil") uint8 NHWC round-half-even(y * 255). */
+int vs_image_postprocess(void* stream, const void* d_x, int nimg, int H, int W, int channels, int format, void* d_out);
+
 /* ---- measurement hooks (bench.py): per-launch CUDA-event timing on the launching stream, by kernel category
- * 0 gemm, 1 conv3x3, 2 spatial/cross attention, 3 temporal attention, 4 groupnorm, 5 layernorm, 6 other.
+ * 0 gemm, 1 conv3x3, 2 spatial/cross attention (and the VAE's row softmax), 3 temporal attention, 4 groupnorm, 5 layernorm,
+ * 6 other.
  * `work` = algorithmic FLOPs (categories 0-2) or algorithmic bytes (3-5) summed over the recorded launches. */
 int vs_profile_enable(int on);
 int vs_profile_reset(void);

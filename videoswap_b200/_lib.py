@@ -112,6 +112,11 @@ _SIGNATURES = {
     "vs_upsample_conv3x3_sized": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _P]),
     "vs_upsample_nearest": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "vs_conv3x3_s2": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P, _P]),
+    "vs_pack_conv_subpixel": (_I, [_P, _P, _I, _I, _P]),
+    "vs_softmax_rows": (_I, [_P, _P, _I, _I, _I, _F]),
+    "vs_transpose_pad": (_I, [_P, _P, _I, _I, _I, _P]),
+    "vs_vae_latent_in": (_I, [_P, _P, _I, _I, _I, _I, _F, _P, _P]),
+    "vs_image_postprocess": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
 }
 
 _lib = None

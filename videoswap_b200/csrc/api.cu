@@ -206,6 +206,24 @@ extern "C" int vs_conv3x3_s2(void* stream, const void* d_x, int nimg, int H, int
   return gemm_tc(st, g);
 }
 
+extern "C" int vs_pack_conv_subpixel(void* stream, const void* d_w, int cout, int cin, void* d_out) {
+  VS_REQUIRE(d_w && d_out, "vs_pack_conv_subpixel: null pointer");
+  return pack_conv_subpixel((cudaStream_t)stream, (const __half*)d_w, cout, cin, (__half*)d_out);
+}
+extern "C" int vs_softmax_rows(void* stream, void* d_s, int rows, int n, int ld, float scale) {
+  return softmax_rows((cudaStream_t)stream, (__half*)d_s, rows, n, ld, scale);
+}
+extern "C" int vs_transpose_pad(void* stream, const void* d_src, int rows, int cols, int rows_pad, void* d_dst) {
+  return transpose_pad((cudaStream_t)stream, (const __half*)d_src, rows, cols, rows_pad, (__half*)d_dst);
+}
+extern "C" int vs_vae_latent_in(void* stream, const void* d_z, int z_is_f32, int nimg, int h, int w, float divisor,
+                                const float* d_wb, void* d_out) {
+  return vae_latent_in((cudaStream_t)stream, d_z, z_is_f32, nimg, h, w, divisor, d_wb, (__half*)d_out);
+}
+extern "C" int vs_image_postprocess(void* stream, const void* d_x, int nimg, int H, int W, int channels, int format, void* d_out) {
+  return image_postprocess((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, channels, format, d_out);
+}
+
 extern "C" int vs_profile_enable(int on) { prof_enable(on != 0); return 0; }
 extern "C" int vs_profile_reset(void) { prof_reset(); return 0; }
 extern "C" int vs_profile_collect(int category, double* ms, double* work, long long* count) {

@@ -507,6 +507,77 @@ int launch_tattn(cudaStream_t st, const TAttnParams& p) {
   return launch_pdl(tattn_kernel<D, FP, true>, dim3((unsigned)blocks), dim3(128), SMEM, st, 1, p);
 }
 
+// ---------------------------------------------------------------------------------------------- single-head attention pieces
+// The VAE mid-block attention (one head, d = 512) runs as GEMMs around these two kernels: S = Q K^T, P = softmax(S), O = P V
+// with V transposed so that both GEMM operands are K-major.
+constexpr int kSoftmaxThreads = 256;
+
+__device__ __forceinline__ float block_reduce(float v, bool is_max, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float w = __shfl_xor_sync(0xffffffffu, v, o);
+    v = is_max ? fmaxf(v, w) : v + w;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();                                   // red[] free (a previous reduction may still be reading it)
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  v = red[0];
+  for (int i = 1; i < kSoftmaxThreads / 32; ++i) v = is_max ? fmaxf(v, red[i]) : v + red[i];
+  return v;
+}
+
+// One block per row of s [rows, ld] fp16, in place: p_j = exp2((s_j - max) sc) / sum_k exp2((s_k - max) sc) for j < n, in
+// fp32 (s_j - max is exact, sc = log2(e) * scale); columns n .. ld - 1 are written 0 and never read.
+__global__ void __launch_bounds__(kSoftmaxThreads) softmax_rows_kernel(__half* __restrict__ s, int n, int ld, float sc) {
+  __shared__ float red[kSoftmaxThreads / 32];
+  uint4* row = reinterpret_cast<uint4*>(s + (long long)blockIdx.x * ld);
+  const int nv = ld / 8;
+  float m = -INFINITY;
+  for (int v = threadIdx.x; v < nv; v += kSoftmaxThreads) {
+    const uint4 x = row[v];
+    const __half* h = reinterpret_cast<const __half*>(&x);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (v * 8 + j < n) m = fmaxf(m, __half2float(h[j]));
+  }
+  m = block_reduce(m, true, red);
+  float l = 0.f;
+  for (int v = threadIdx.x; v < nv; v += kSoftmaxThreads) {
+    const uint4 x = row[v];
+    const __half* h = reinterpret_cast<const __half*>(&x);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      if (v * 8 + j < n) l += exp2f((__half2float(h[j]) - m) * sc);
+  }
+  l = block_reduce(l, false, red);
+  for (int v = threadIdx.x; v < nv; v += kSoftmaxThreads) {
+    const uint4 x = row[v];
+    const __half* h = reinterpret_cast<const __half*>(&x);
+    uint4 o;
+    __half* oh = reinterpret_cast<__half*>(&o);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      oh[j] = v * 8 + j < n ? __float2half_rn(exp2f((__half2float(h[j]) - m) * sc) / l) : __float2half_rn(0.f);
+    row[v] = o;
+  }
+}
+
+// dst [cols, rows_pad] = src [rows, cols]^T, columns rows .. rows_pad - 1 of dst zero.  32 x 32 tiles through shared memory.
+__global__ void transpose_pad_kernel(const __half* __restrict__ src, int rows, int cols, int rows_pad, __half* __restrict__ dst) {
+  __shared__ __half tile[32][33];
+  const int r0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int r = r0 + j, c = c0 + threadIdx.x;
+    if (c < cols) tile[j][threadIdx.x] = r < rows ? src[(long long)r * cols + c] : __float2half_rn(0.f);
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int c = c0 + j, r = r0 + threadIdx.x;
+    if (c < cols && r < rows_pad) dst[(long long)c * rows_pad + r] = tile[threadIdx.x][j];
+  }
+}
+
 }  // namespace
 
 int attention(cudaStream_t st, const __half* q, int ldq, const __half* k, int ldk, const __half* v, int ldv, __half* o,
@@ -568,6 +639,22 @@ int temporal_attention(cudaStream_t st, const __half* qkv, __half* o, int B, int
     case 160: return big ? launch_tattn<160, 32>(st, p) : launch_tattn<160, 16>(st, p);
     default: VS_REQUIRE(false, "temporal_attention: unsupported head dim %d", d);
   }
+}
+
+int softmax_rows(cudaStream_t st, __half* s, int rows, int n, int ld, float scale) {
+  VS_REQUIRE(s && rows > 0 && n > 0 && n <= ld && ld % 8 == 0, "softmax_rows: bad shape (rows %d, n %d, ld %d)", rows, n, ld);
+  ProfScope prof(st, PC_ATTN, 5.0 * rows * (double)n);   // max, subtract, scale, exp, divide per element
+  softmax_rows_kernel<<<rows, kSoftmaxThreads, 0, st>>>(s, n, ld, 1.4426950408889634f * scale);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int transpose_pad(cudaStream_t st, const __half* src, int rows, int cols, int rows_pad, __half* dst) {
+  VS_REQUIRE(src && dst && rows > 0 && cols > 0 && rows_pad >= rows, "transpose_pad: bad shape (%d x %d, pad %d)", rows, cols, rows_pad);
+  ProfScope prof(st, PC_OTHER, 2.0 * ((double)rows + rows_pad) * cols);    // bytes read + written
+  transpose_pad_kernel<<<dim3((rows_pad + 31) / 32, (cols + 31) / 32), dim3(32, 8), 0, st>>>(src, rows, cols, rows_pad, dst);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace vs

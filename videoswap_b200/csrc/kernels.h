@@ -93,6 +93,11 @@ int set_option(const char* name, int value);
 int get_option(const char* name);
 // Temporal attention across F frames per pixel: qkv [B, F, HW, 3C] -> o [B, F, HW, C].
 int temporal_attention(cudaStream_t st, const __half* qkv, __half* o, int B, int F, int HW, int C, int heads);
+// Row softmax of s [rows, ld] fp16 in place over the first n columns (fp32 math, logits s * scale); columns n .. ld - 1
+// are set to 0.  ld % 8 == 0.
+int softmax_rows(cudaStream_t st, __half* s, int rows, int n, int ld, float scale);
+// dst [cols, rows_pad] = src [rows, cols]^T with zero columns rows .. rows_pad - 1.
+int transpose_pad(cudaStream_t st, const __half* src, int rows, int cols, int rows_pad, __half* dst);
 
 // ---- pointwise / small -----------------------------------------------------------------------------------------
 int small_linear(cudaStream_t st, const float* x, int rows, int K, const __half* W, const float* bias, int N,
@@ -108,6 +113,12 @@ int add_inplace(cudaStream_t st, __half* x, const __half* r, size_t n, float sca
 int ncfhw_to_nhwc(cudaStream_t st, const void* src, int src_is_f32, int B, int C, int F, int H, int W, __half* dst);
 int nhwc_to_ncfhw(cudaStream_t st, const __half* src, int B, int C, int F, int H, int W, void* dst, int dst_is_f32);
 int nchw_to_nhwc(cudaStream_t st, const __half* src, int n, int C, int H, int W, float scale, __half* dst);
+// VAE decoder entry: post_quant_conv(z / divisor), z NCHW [nimg, 4, h, w] (fp16, or fp32 with z_is_f32) -> NHWC fp16
+// [nimg, h, w, 4]; wb fp32 = weight [4][4] then bias [4].
+int vae_latent_in(cudaStream_t st, const void* z, int z_is_f32, int nimg, int h, int w, float divisor, const float* wb, __half* out);
+// VAE decoder exit: channels 0..2 of NHWC fp16 x [nimg, H, W, cs] (cs % 8 == 0) in one of the formats below.
+enum ImageFormat { IMG_SAMPLE = 0, IMG_PT = 1, IMG_NP = 2, IMG_PIL = 3 };
+int image_postprocess(cudaStream_t st, const __half* x, int nimg, int H, int W, int cs, int format, void* out);
 // eps = u + s (c - u); x_prev = sqrt(a_p) (x - sqrt(1-a_t) eps)/sqrt(a_t) + sqrt(1-a_p) eps.  eps2: [2, n] (uncond
 // first) or [1, n] when guidance is disabled (cfg == 0).
 int cfg_ddim_step(cudaStream_t st, const void* eps2, const void* latents, int is_f32, size_t n, int cfg,

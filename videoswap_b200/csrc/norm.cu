@@ -282,7 +282,9 @@ int gn_fill(GnParams& p, dim3& grid, int& threads, const __half* x1, int c1, con
   const int C = c1 + c2;
   VS_REQUIRE(x1 && c1 > 0 && (c2 == 0 || x2), "groupnorm: bad inputs");
   VS_REQUIRE(c1 % 8 == 0 && c2 % 8 == 0, "groupnorm: channel counts must be multiples of 8 (got %d, %d)", c1, c2);
-  VS_REQUIRE(C % groups == 0 && (C / groups) >= 8, "groupnorm: needs >= 8 channels per group (C=%d groups=%d)", C, groups);
+  // every thread's 8-channel vector must lie in at most two groups (ga / gb of the statistics kernel): 4 or >= 8 per group
+  VS_REQUIRE(C % groups == 0 && ((C / groups) == 4 || (C / groups) >= 8),
+             "groupnorm: needs 4 or >= 8 channels per group (C=%d groups=%d)", C, groups);
   VS_REQUIRE(nimg % imgs_per_set == 0, "groupnorm: nimg %% imgs_per_set != 0");
   VS_REQUIRE(C / 8 <= 1024, "groupnorm: too many channels");
   p.x1 = x1; p.x2 = x2; p.c1 = c1; p.c2 = c2; p.C = C; p.CV = C / 8;

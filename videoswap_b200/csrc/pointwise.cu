@@ -480,6 +480,53 @@ __global__ void __launch_bounds__(128) ln_fold_kernel(const __half* __restrict__
   }
 }
 
+// ---------------------------------------------------------------------------------------------- VAE decoder entry / exit
+// post_quant_conv(z / divisor) (diffusers AutoencoderKL._decode): NCHW [n, 4, h, w] fp16 or fp32 latents -> NHWC fp16 [n, h, w, 4].
+// wb: fp32 [4][4] weight then [4] bias.  Fixed order, no contraction: out_c = (((b_c + w_c0 x_0) + w_c1 x_1) + w_c2 x_2) + w_c3 x_3.
+template <typename T>
+__global__ void vae_latent_in_kernel(const T* __restrict__ z, long long npix, int hw, float divisor, const float* __restrict__ wb,
+                                     __half* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
+    const long long img = i / hw, p = i % hw;
+    float x[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) x[k] = (float)z[(img * 4 + k) * hw + p] / divisor;
+    __half o[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      float acc = wb[16 + c];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) acc = __fadd_rn(acc, __fmul_rn(wb[c * 4 + k], x[k]));
+      o[c] = __float2half_rn(acc);
+    }
+    *reinterpret_cast<uint2*>(out + i * 4) = *reinterpret_cast<const uint2*>(o);
+  }
+}
+
+// VaeImageProcessor.postprocess of channels 0..2 of the decoder's NHWC fp16 output x [n, H, W, cs]:
+//   IMG_SAMPLE  x itself as fp16 NCHW [n, 3, H, W] (AutoencoderKL.decode's sample, not denormalised)
+//   IMG_PT      y = clamp(x / 2 + 0.5, 0, 1) as fp32 NCHW;  IMG_NP  y as fp32 NHWC [n, H, W, 3]
+//   IMG_PIL     uint8 NHWC round_half_even(y * 255) (numpy's round, then astype(uint8))
+__global__ void image_postprocess_kernel(const __half* __restrict__ x, long long npix, int hw, int cs, int format, void* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = *reinterpret_cast<const uint4*>(x + i * cs);
+    const __half* h = reinterpret_cast<const __half*>(&v);
+    const long long img = i / hw, p = i % hw;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const long long nchw = (img * 3 + c) * hw + p;
+      if (format == IMG_SAMPLE) {
+        reinterpret_cast<__half*>(out)[nchw] = h[c];
+        continue;
+      }
+      const float y = fminf(fmaxf(__fadd_rn(__fmul_rn(__half2float(h[c]), 0.5f), 0.5f), 0.f), 1.f);
+      if (format == IMG_PT) reinterpret_cast<float*>(out)[nchw] = y;
+      else if (format == IMG_NP) reinterpret_cast<float*>(out)[i * 3 + c] = y;
+      else reinterpret_cast<uint8_t*>(out)[i * 3 + c] = (uint8_t)__float2int_rn(__fmul_rn(y, 255.f));
+    }
+  }
+}
+
 inline unsigned capped(size_t n) {
   size_t b = (n + TPB - 1) / TPB;
   const size_t cap = (size_t)num_sms() * 16;
@@ -646,6 +693,26 @@ int ln_fold(cudaStream_t st, const __half* w, int N, int K, const float* gamma, 
   VS_REQUIRE(!pe || cpe, "ln_fold: positional table without an output");
   ln_fold_kernel<<<N, 128, 0, st>>>(w, N, K, gamma, beta, bias, pe, pe ? pe_len : 0, wf, u, c, cpe);
   count_launch(1);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+int vae_latent_in(cudaStream_t st, const void* z, int z_is_f32, int nimg, int h, int w, float divisor, const float* wb, __half* out) {
+  VS_REQUIRE(z && wb && out && nimg > 0 && h > 0 && w > 0 && divisor != 0.f, "vae_latent_in: bad arguments");
+  const long long npix = (long long)nimg * h * w;
+  ProfScope prof(st, PC_OTHER, (double)npix * (4 * (z_is_f32 ? 4 : 2) + 8));   // bytes read + written
+  if (z_is_f32) vae_latent_in_kernel<float><<<capped((size_t)npix), TPB, 0, st>>>((const float*)z, npix, h * w, divisor, wb, out);
+  else vae_latent_in_kernel<__half><<<capped((size_t)npix), TPB, 0, st>>>((const __half*)z, npix, h * w, divisor, wb, out);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+int image_postprocess(cudaStream_t st, const __half* x, int nimg, int H, int W, int cs, int format, void* out) {
+  VS_REQUIRE(x && out && nimg > 0 && H > 0 && W > 0, "image_postprocess: bad arguments");
+  VS_REQUIRE(cs >= 8 && cs % 8 == 0, "image_postprocess: the input's channel count must be a multiple of 8 (got %d)", cs);
+  VS_REQUIRE(format >= IMG_SAMPLE && format <= IMG_PIL, "image_postprocess: unknown format %d", format);
+  const long long npix = (long long)nimg * H * W;
+  const int out_bytes = format == IMG_PIL ? 3 : (format == IMG_SAMPLE ? 6 : 12);
+  ProfScope prof(st, PC_OTHER, (double)npix * (16 + out_bytes));
+  image_postprocess_kernel<<<capped((size_t)npix), TPB, 0, st>>>(x, npix, H * W, cs, format, out);
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -156,6 +156,29 @@ def upsample_conv3x3(x, w, bias=None):
     return out
 
 
+def pack_conv_subpixel(w):
+    """[Co, Ci, 3, 3] fp16 -> the four sub-pixel panels of upsample_conv3x3, [4 parities (py * 2 + px), Co, 4 * Ci]."""
+    _chk16(w)
+    co, ci = w.shape[:2]
+    out = torch.empty((4, co, 4 * ci), dtype=torch.float16, device=w.device)
+    _lib.call("vs_pack_conv_subpixel", _stream(), _p(w), co, ci, _p(out))
+    return out
+
+
+def upsample_conv3x3_packed(x, wsub, bias=None):
+    """upsample_conv3x3 on panels from pack_conv_subpixel: one tensor-core launch per output parity."""
+    _chk16(x, wsub)
+    _chk32(bias)
+    n, H, W, Ci = x.shape
+    co = wsub.shape[1]
+    assert tuple(wsub.shape) == (4, co, 4 * Ci), "expected pack_conv_subpixel panels"
+    out = torch.empty((n, 2 * H, 2 * W, co), dtype=torch.float16, device=x.device)
+    for par in range(4):
+        _gemm_ex(A=_ptr(x), K1=Ci, lda1=Ci, Bw=_ptr(wsub[par]), M=n * H * W, N=co, taps=4, sub_py=par >> 1, sub_px=par & 1,
+                 nimg=n, H=H, W=W, bias=_ptr(bias), out=_ptr(out), ldc=co)
+    return out
+
+
 def upsample_conv3x3_sized(x, w, bias, OH, OW, out=None):
     """nearest up-sampling to OH x OW (2H or 2H - 1 rows, 2W or 2W - 1 columns) + conv3x3 (pad 1), as the UNet's up path
     runs it: x [N, H, W, C], w [Co, C, 3, 3] (unpacked) -> [N, OH, OW, Co].  `out` may be any contiguous fp16 buffer of at
@@ -299,6 +322,61 @@ def attention_apply_probs(probs, v, heads, kv_div=1):
     out = torch.empty((B, nq, Cc), dtype=torch.float16, device=probs.device)
     _lib.call("vs_attention_apply_probs", _stream(), _p(probs), _p(v), v.stride(1), _p(out), Cc, B, nq, nk, heads, Cc // heads,
               v.stride(0), nq * Cc, kv_div)
+    return out
+
+
+def scores(q, k, out):
+    """out[i, j] = q_i . k_j (fp16) for q [nq, d], k [nk, d]; out [nq, ld] with ld >= nk (columns nk .. ld - 1 untouched)."""
+    _chk16(q, k, out)
+    nq, d = q.shape
+    nk = k.shape[0]
+    assert k.shape[1] == d and out.dim() == 2 and out.shape[0] == nq and out.shape[1] >= nk
+    _gemm_ex(A=_ptr(q), K1=d, lda1=d, Bw=_ptr(k), M=nq, N=nk, out=_ptr(out), ldc=out.shape[1])
+    return out
+
+
+def softmax_rows(s, n, scale):
+    """In place on s [rows, ld] fp16: softmax(s * scale) over the first n columns (fp32 math), zeros in columns n .. ld - 1."""
+    _chk16(s)
+    rows, ld = s.shape
+    _lib.call("vs_softmax_rows", _stream(), _p(s), rows, n, ld, float(scale))
+    return s
+
+
+def transpose_pad(x, rows_pad, out=None):
+    """x [rows, cols] fp16 -> [cols, rows_pad] = x^T with zero columns rows .. rows_pad - 1."""
+    _chk16(x)
+    rows, cols = x.shape
+    out = _out16(out, (cols, rows_pad), x.device)
+    _lib.call("vs_transpose_pad", _stream(), _p(x), rows, cols, rows_pad, _p(out))
+    return out
+
+
+def vae_latent_in(z, divisor, wb):
+    """post_quant_conv(z / divisor): z [n, 4, h, w] fp16 / fp32 NCHW, wb fp32 [20] (weight [4, 4], then bias [4]) ->
+    NHWC fp16 [n, h, w, 4]."""
+    assert z.is_cuda and z.dtype in (torch.float16, torch.float32) and z.is_contiguous() and z.dim() == 4 and z.shape[1] == 4, \
+        "expected contiguous [n, 4, h, w] fp16 / fp32 CUDA latents"
+    _chk32(wb)
+    assert wb.numel() == 20
+    n, _, h, w = z.shape
+    out = torch.empty((n, h, w, 4), dtype=torch.float16, device=z.device)
+    _lib.call("vs_vae_latent_in", _stream(), _p(z), int(z.dtype == torch.float32), n, h, w, float(divisor), _p(wb), _p(out))
+    return out
+
+
+IMG_SAMPLE, IMG_PT, IMG_NP, IMG_PIL = 0, 1, 2, 3
+
+
+def image_postprocess(x, fmt):
+    """Channels 0..2 of the decoder output x [n, H, W, C] (C % 8 == 0): IMG_SAMPLE fp16 [n, 3, H, W] as is; else
+    y = clamp(x / 2 + 0.5, 0, 1) as IMG_PT fp32 [n, 3, H, W], IMG_NP fp32 [n, H, W, 3] or IMG_PIL uint8 [n, H, W, 3]."""
+    _chk16(x)
+    n, H, W, Cc = x.shape
+    shape = (n, 3, H, W) if fmt in (IMG_SAMPLE, IMG_PT) else (n, H, W, 3)
+    dtype = {IMG_SAMPLE: torch.float16, IMG_PT: torch.float32, IMG_NP: torch.float32, IMG_PIL: torch.uint8}[fmt]
+    out = torch.empty(shape, dtype=dtype, device=x.device)
+    _lib.call("vs_image_postprocess", _stream(), _p(x), n, H, W, Cc, fmt, _p(out))
     return out
 
 

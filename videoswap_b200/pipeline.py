@@ -2,9 +2,9 @@
 denoising part of `VideoSwapPipeline` (videoswap/pipelines/pipeline_videoswap.py:427-619 `__call__`, :622-721 `invert`).
 
 Scope (SURVEY.md 8): the loop body -- CFG batch duplication, UNet forward, CFG combine, scheduler step, adapter
-residual window -- runs on the native kernels.  Text encoding (CLIP), VAE encode/decode, prompt/LoRA handling and the
-attention controllers are callers on either side of this path (8f) and are NOT part of this package: the pipeline
-takes `prompt_embeds` / `latents` tensors and returns latents.
+residual window -- runs on the native kernels.  Text encoding (CLIP), VAE encode and prompt/LoRA handling are callers on
+either side of this path (8f) and are NOT part of this package: the pipeline takes `prompt_embeds` / `latents` tensors and
+returns latents, or, given a `vae` (videoswap_b200.vae.AutoencoderKL), the decoded frames.
 """
 from __future__ import annotations
 
@@ -18,6 +18,7 @@ from . import ops
 from .scheduler import DDIMInverseScheduler, DDIMScheduler
 from .spec import adapter_param_shapes
 from .unet import AnimateDiffUNet3DModel, _Holder
+from .vae import AutoencoderKL
 from .weights import seeded_state_dict
 
 
@@ -95,11 +96,15 @@ class VideoSwapPipeline:
     """The denoising loop of the reference pipeline on the native path.  BASELINE.json's `TuneAVideoPipeline` alias."""
 
     def __init__(self, unet: AnimateDiffUNet3DModel, scheduler: Optional[DDIMScheduler] = None,
-                 adapter: Optional[SparsePointAdapter] = None, inverse_scheduler: Optional[DDIMInverseScheduler] = None):
+                 adapter: Optional[SparsePointAdapter] = None, inverse_scheduler: Optional[DDIMInverseScheduler] = None,
+                 vae: Optional[AutoencoderKL] = None):
+        """vae: the decoder that turns the final latents into frames (output_type "pt" / "np" / "pil"); without it the
+        pipeline returns latents only."""
         self.unet = unet
         self.scheduler = scheduler or DDIMScheduler()
         self.inverse_scheduler = inverse_scheduler or DDIMInverseScheduler()
         self.adapter = adapter
+        self.vae = vae
 
     @property
     def device(self):
@@ -154,9 +159,13 @@ class VideoSwapPipeline:
                  output_type: str = "latent", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_iters: Optional[int] = None):
         """prompt_embeds: [1,77,D] / ED-LoRA [1,16,77,D] (conditional); negative_prompt_embeds same shape (uncond).
-        latents [1,4,F,h,w] (e.g. DDIM-inverted).  Mirrors pipeline_videoswap.py:552-601."""
+        latents [1,4,F,h,w] (e.g. DDIM-inverted).  Mirrors pipeline_videoswap.py:552-610: output_type "latent" returns
+        the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents)."""
         if output_type != "latent":
-            raise NotImplementedError("VAE decode is outside the hot path (SURVEY 8f-4); use output_type='latent'")
+            if self.vae is None:
+                raise NotImplementedError("decoding needs a VideoSwapPipeline(..., vae=AutoencoderKL); use output_type='latent'")
+            if output_type not in ("pt", "np", "pil"):
+                raise ValueError(f"output_type must be 'latent', 'pt', 'np' or 'pil', got {output_type!r}")
         cfg = guidance_scale > 1.0
         dev = latents.device
         if cfg:
@@ -194,9 +203,23 @@ class VideoSwapPipeline:
         # the reference always rearranges 'b c f h w -> (b f) c h w' before returning (pipeline_videoswap.py:603-610)
         b, c, f, h, w = latents.shape
         video = latents.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
+        if output_type != "latent":
+            video = self.decode_latents(video, output_type)
         if not return_dict:
             return video
         return TuneAVideoPipelineOutput(videos=video)
+
+    @torch.no_grad()
+    def decode_latents(self, latents: torch.Tensor, output_type: str = "pil"):
+        """Frames of latents [(b f), 4, h, w] (or [b, 4, f, h, w]): image_processor.postprocess(vae.decode(latents /
+        scaling_factor)) as pipeline_videoswap.py:603-610 computes it.  "pt": fp32 [(b f), 3, 8h, 8w] in [0, 1]; "np": fp32
+        numpy [(b f), 8h, 8w, 3]; "pil": a list of RGB PIL images."""
+        if self.vae is None:
+            raise NotImplementedError("decoding needs a VideoSwapPipeline(..., vae=AutoencoderKL)")
+        if latents.dim() == 5:
+            b, c, f, h, w = latents.shape
+            latents = latents.permute(0, 2, 1, 3, 4).reshape(b * f, c, h, w)
+        return self.vae.decode_postprocess(latents, output_type)
 
     @torch.no_grad()
     def invert(self, prompt_embeds: torch.Tensor, latents: torch.Tensor, num_inference_steps: int = 50,

@@ -184,6 +184,67 @@ def unet_param_shapes(cfg: UNetConfig) -> "OrderedDict[str, Tuple[int, ...]]":
     return sh
 
 
+@dataclass
+class VAEConfig:
+    """The decoder side of diffusers 0.19.3 AutoencoderKL as SD-1.5 configures it (vae/config.json)."""
+    in_channels: int = 3
+    out_channels: int = 3
+    block_out_channels: Tuple[int, ...] = (128, 256, 512, 512)
+    layers_per_block: int = 2
+    latent_channels: int = 4
+    norm_num_groups: int = 32
+    scaling_factor: float = 0.18215
+    sample_size: int = 512
+
+    def to_dict(self):
+        return asdict(self)
+
+
+def _vae_resnet(sh, p, cin, cout):
+    """ResnetBlock2D with temb_channels=None (no time_emb_proj)."""
+    for n, c in (("norm1", cin), ("norm2", cout)):
+        _norm(sh, f"{p}.{n}", c)
+    sh[p + ".conv1.weight"] = (cout, cin, 3, 3)
+    sh[p + ".conv1.bias"] = (cout,)
+    sh[p + ".conv2.weight"] = (cout, cout, 3, 3)
+    sh[p + ".conv2.bias"] = (cout,)
+    if cin != cout:
+        sh[p + ".conv_shortcut.weight"] = (cout, cin, 1, 1)
+        sh[p + ".conv_shortcut.bias"] = (cout,)
+
+
+def vae_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...]]":
+    """Decoder-side AutoencoderKL state_dict (diffusers 0.19.3 names: the mid-block attention as to_q / to_k / to_v /
+    to_out.0).  The encoder and quant_conv are not part of it."""
+    sh: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    lc, boc = cfg.latent_channels, list(cfg.block_out_channels)
+    sh["post_quant_conv.weight"] = (lc, lc, 1, 1)
+    sh["post_quant_conv.bias"] = (lc,)
+    c = boc[-1]
+    sh["decoder.conv_in.weight"] = (c, lc, 3, 3)
+    sh["decoder.conv_in.bias"] = (c,)
+    _vae_resnet(sh, "decoder.mid_block.resnets.0", c, c)
+    a = "decoder.mid_block.attentions.0"
+    _norm(sh, a + ".group_norm", c)
+    for n in ("to_q", "to_k", "to_v", "to_out.0"):
+        sh[f"{a}.{n}.weight"] = (c, c)
+        sh[f"{a}.{n}.bias"] = (c,)
+    _vae_resnet(sh, "decoder.mid_block.resnets.1", c, c)
+    rev = boc[::-1]
+    prev = rev[0]
+    for i, out in enumerate(rev):
+        for j in range(cfg.layers_per_block + 1):
+            _vae_resnet(sh, f"decoder.up_blocks.{i}.resnets.{j}", prev if j == 0 else out, out)
+        if i < len(rev) - 1:
+            sh[f"decoder.up_blocks.{i}.upsamplers.0.conv.weight"] = (out, out, 3, 3)
+            sh[f"decoder.up_blocks.{i}.upsamplers.0.conv.bias"] = (out,)
+        prev = out
+    _norm(sh, "decoder.conv_norm_out", boc[0])
+    sh["decoder.conv_out.weight"] = (cfg.out_channels, boc[0], 3, 3)
+    sh["decoder.conv_out.bias"] = (cfg.out_channels,)
+    return sh
+
+
 def adapter_param_shapes(embedding_channels=1280, channels=(320, 640, 1280, 1280), mid_dim=128):
     """SparsePointAdapter state_dict (videoswap/models/adapter_model.py:50-70 of the reference)."""
     sh = OrderedDict()

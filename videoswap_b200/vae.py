@@ -1,0 +1,267 @@
+"""The decoder half of diffusers 0.19.3 `AutoencoderKL` (SD-1.5's VAE) on the native kernels, with the decoder-side
+config and state_dict names of diffusers.  The reference's loop ends with `vae.decode(latents / scaling_factor)` and
+`VaeImageProcessor.postprocess` (videoswap/pipelines/pipeline_videoswap.py:603-610); `decode_postprocess` replaces the two
+calls, `decode` the first.
+
+Executor: a short sequence over `ops`, activations NHWC fp16, every frame of a call in one pass (the GroupNorms are per
+image, so frames stay independent).  The mid block's single-head attention (d = 512) runs per frame as GEMMs around a row
+softmax: S = Q K^T into one [hw, hw_pad] buffer, P = softmax(S / sqrt(512)) in place, O = P V with V transposed."""
+from __future__ import annotations
+
+import json
+import math
+import os
+from dataclasses import dataclass, fields
+from typing import Dict, Optional
+
+import torch
+
+from . import ops
+from .spec import VAEConfig, vae_param_shapes
+from .weights import seeded_state_dict
+
+EPS = 1e-6                     # resnet_eps of the SD-1.5 decoder (GroupNorms of resnets, attention and conv_norm_out)
+CONV_OUT_PAD = 8               # conv_out's 3 output channels padded to 8 so the conv kernel's stores stay 16-byte aligned
+
+# Pre-0.14 diffusers names of the mid-block attention, still shipped in SD-1.5 VAE files ([C, C] or 1x1-conv [C, C, 1, 1])
+_OLD_ATTN = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
+_IGNORED_PREFIXES = ("encoder.", "quant_conv.")   # the encode half: accepted so that a whole VAE file loads
+
+
+@dataclass
+class DecoderOutput:
+    sample: torch.Tensor
+
+
+def convert_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str, torch.Tensor]:
+    """A full or decoder-only AutoencoderKL state_dict -> the decoder keys of vae_param_shapes(cfg), in their shapes.
+    Old attention names are renamed, encoder / quant_conv keys dropped; any other unknown key, a wrong shape or a missing
+    decoder key raises."""
+    shapes = vae_param_shapes(cfg)
+    out = {}
+    for k, v in sd.items():
+        if k.startswith(_IGNORED_PREFIXES):
+            continue
+        name = k
+        head, _, leaf = k.rpartition(".")
+        attn, _, old = head.rpartition(".")
+        if attn == "decoder.mid_block.attentions.0" and old in _OLD_ATTN:
+            name = f"{attn}.{_OLD_ATTN[old]}.{leaf}"
+        if name not in shapes:
+            raise KeyError(f"unexpected key in the VAE state_dict: {k}")
+        if name in out:
+            raise KeyError(f"{k}: {name} is given twice (old and new attention names)")
+        want = shapes[name]
+        if tuple(v.shape) != want:
+            if name.startswith(attn + ".") and len(want) == 2 and tuple(v.shape) == want + (1, 1):
+                v = v.reshape(want)
+            else:
+                raise ValueError(f"{k}: shape {tuple(v.shape)}, expected {want}")
+        out[name] = v
+    missing = [k for k in shapes if k not in out]
+    if missing:
+        raise KeyError(f"missing decoder keys in the VAE state_dict: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
+    return out
+
+
+def padded_keys(nk: int) -> int:
+    """Row stride of S / P: O = P V runs with K = this, which the GEMM needs to be a multiple of 8."""
+    return -(-nk // 8) * 8
+
+
+def attend(q, k, v, s, vt, out):
+    """One frame of single-head attention, out = softmax(q k^T / sqrt(d)) v: q, k, v [hw, d] fp16; scratch s
+    [hw, padded_keys(hw)] (S, then P in place) and vt [d, padded_keys(hw)] (V^T with zero padding columns)."""
+    hw, d = q.shape
+    ops.scores(q, k, s)
+    ops.softmax_rows(s, hw, 1.0 / math.sqrt(d))
+    ops.transpose_pad(v, s.shape[1], out=vt)
+    return ops.gemm(s, vt, out=out)
+
+
+class AutoencoderKL:
+    """Decoder side of diffusers' AutoencoderKL on CUDA.  init="seeded" draws test weights (weights.seeded_state_dict),
+    "empty" waits for load_state_dict."""
+
+    def __init__(self, init: str = "seeded", device="cuda", **config):
+        self.config = VAEConfig(**config)
+        cfg = self.config
+        if cfg.latent_channels != 4 or cfg.out_channels != 3:
+            raise ValueError("the native decoder takes 4 latent channels and makes 3 image channels")
+        self.device = torch.device(device)
+        self._w = None
+        if init == "seeded":
+            self.load_state_dict(seeded_state_dict(vae_param_shapes(cfg), seed=7))
+        elif init != "empty":
+            raise ValueError(f"init must be 'seeded' or 'empty', got {init!r}")
+
+    # ------------------------------------------------------------------------------------------------ construction
+    @classmethod
+    def from_config(cls, config, **kw):
+        """diffusers-style: keys of VAEConfig are used, the rest of a config.json (class name, block types, ...) ignored."""
+        if not isinstance(config, dict):
+            config = config.to_dict()
+        if config.get("act_fn", "silu") != "silu":
+            raise ValueError(f"unsupported act_fn {config['act_fn']!r}")
+        known = {f.name for f in fields(VAEConfig)}
+        return cls(**kw, **{k: (tuple(v) if isinstance(v, list) else v) for k, v in config.items() if k in known})
+
+    @classmethod
+    def from_pretrained(cls, path: str, subfolder: Optional[str] = "vae", device="cuda"):
+        """A local diffusers directory: config.json + diffusion_pytorch_model.safetensors (or .bin)."""
+        d = os.path.join(path, subfolder) if subfolder else path
+        cfg_path = os.path.join(d, "config.json")
+        if not os.path.exists(cfg_path):
+            raise RuntimeError(f"{cfg_path} not found")
+        with open(cfg_path) as f:
+            m = cls.from_config(json.load(f), init="empty", device=device)
+        st, bn = os.path.join(d, "diffusion_pytorch_model.safetensors"), os.path.join(d, "diffusion_pytorch_model.bin")
+        if os.path.exists(st):
+            from safetensors.torch import load_file
+            sd = load_file(st)
+        elif os.path.exists(bn):
+            sd = torch.load(bn, map_location="cpu", weights_only=True)
+        else:
+            raise RuntimeError(f"no diffusion_pytorch_model.safetensors / .bin in {d}")
+        m.load_state_dict(sd)
+        return m
+
+    # ------------------------------------------------------------------------------------------------ weights
+    def load_state_dict(self, sd: Dict[str, torch.Tensor]):
+        """Converts (convert_state_dict) and packs every weight once: conv3x3 panels, sub-pixel panels of the up-samplers,
+        the attention's q / k / v as one [3C, C] weight, conv_out padded to 8 output channels."""
+        if self.device.type != "cuda":
+            raise RuntimeError("AutoencoderKL (videoswap_b200) runs on CUDA only")
+        sd = convert_state_dict(sd, self.config)
+        dev = self.device
+        h16 = lambda k: sd[k].detach().to(dev, torch.float16).contiguous()
+        f32 = lambda k: sd[k].detach().to(dev, torch.float32).contiguous()
+
+        def norm(p):
+            return f32(p + ".weight"), f32(p + ".bias")
+
+        def resnet(p):
+            r = {"norm1": norm(p + ".norm1"), "norm2": norm(p + ".norm2"),
+                 "conv1": (ops.pack_conv3x3(h16(p + ".conv1.weight")), f32(p + ".conv1.bias")),
+                 "conv2": (ops.pack_conv3x3(h16(p + ".conv2.weight")), f32(p + ".conv2.bias"))}
+            if p + ".conv_shortcut.weight" in sd:
+                w = h16(p + ".conv_shortcut.weight")
+                r["shortcut"] = (w.reshape(w.shape[0], w.shape[1]).contiguous(), f32(p + ".conv_shortcut.bias"))
+            return r
+
+        a = "decoder.mid_block.attentions.0"
+        cfg = self.config
+        n_up = len(cfg.block_out_channels)
+        w = {
+            "latent_in": torch.cat([f32("post_quant_conv.weight").flatten(), f32("post_quant_conv.bias")]).contiguous(),
+            "conv_in": (h16("decoder.conv_in.weight"), f32("decoder.conv_in.bias")),
+            "mid": [resnet(f"decoder.mid_block.resnets.{j}") for j in (0, 1)],
+            "attn": {"norm": norm(a + ".group_norm"),
+                     "qkv": (torch.cat([h16(f"{a}.{n}.weight") for n in ("to_q", "to_k", "to_v")]).contiguous(),
+                             torch.cat([f32(f"{a}.{n}.bias") for n in ("to_q", "to_k", "to_v")]).contiguous()),
+                     "out": (h16(a + ".to_out.0.weight"), f32(a + ".to_out.0.bias"))},
+            "up": [{"resnets": [resnet(f"decoder.up_blocks.{i}.resnets.{j}") for j in range(cfg.layers_per_block + 1)],
+                    "upsampler": (ops.pack_conv_subpixel(h16(f"decoder.up_blocks.{i}.upsamplers.0.conv.weight")),
+                                  f32(f"decoder.up_blocks.{i}.upsamplers.0.conv.bias")) if i < n_up - 1 else None}
+                   for i in range(n_up)],
+            "norm_out": norm("decoder.conv_norm_out"),
+        }
+        wo = torch.zeros((CONV_OUT_PAD,) + tuple(sd["decoder.conv_out.weight"].shape[1:]), dtype=torch.float16, device=dev)
+        wo[:cfg.out_channels] = h16("decoder.conv_out.weight")
+        bo = torch.zeros(CONV_OUT_PAD, dtype=torch.float32, device=dev)
+        bo[:cfg.out_channels] = f32("decoder.conv_out.bias")
+        w["conv_out"] = (ops.pack_conv3x3(wo), bo)
+        self._w = w
+        return self
+
+    # ------------------------------------------------------------------------------------------------ executor
+    def _groups(self):
+        return self.config.norm_num_groups
+
+    def _resnet(self, x, r):
+        """ResnetBlock2D with temb=None: conv2(silu(gn2(conv1(silu(gn1(x)))))) + shortcut(x), output_scale_factor 1."""
+        n, H, W, ci = x.shape
+        h = ops.groupnorm(x, *r["norm1"], self._groups(), EPS, silu=True)
+        h = ops.conv3x3(h, *r["conv1"])
+        h = ops.groupnorm(h, *r["norm2"], self._groups(), EPS, silu=True)
+        sc = x
+        if "shortcut" in r:
+            ws, bs = r["shortcut"]
+            sc = ops.gemm(x.view(n * H * W, ci), ws, bias=bs).view(n, H, W, ws.shape[0])
+        return ops.conv3x3(h, *r["conv2"], residual=sc)
+
+    def _attention(self, x, a):
+        """Attention(heads=1, residual_connection=True) under AttnProcessor2_0: to_out(softmax(q k^T / sqrt(C)) v) + x."""
+        n, H, W, C = x.shape
+        hw = H * W
+        ld = padded_keys(hw)
+        h = ops.groupnorm(x, *a["norm"], self._groups(), EPS).view(n * hw, C)
+        wqkv, bqkv = a["qkv"]
+        # q, k, v from row blocks of the packed weight, each its own contiguous tensor: K is the B operand of S = Q K^T,
+        # which the GEMM reads with unit-stride rows
+        q, k, v = (ops.gemm(h, wqkv[i * C:(i + 1) * C], bias=bqkv[i * C:(i + 1) * C]) for i in range(3))
+        s = torch.empty((hw, ld), dtype=torch.float16, device=x.device)
+        vt = torch.empty((C, ld), dtype=torch.float16, device=x.device)
+        o = torch.empty((n * hw, C), dtype=torch.float16, device=x.device)
+        for f in range(n):
+            rows = slice(f * hw, (f + 1) * hw)
+            attend(q[rows], k[rows], v[rows], s, vt, o[rows])
+        wo, bo = a["out"]
+        return ops.gemm(o, wo, bias=bo, residual=x.view(n * hw, C)).view(n, H, W, C)
+
+    def _run(self, z, divisor, fmt, taps=None):
+        """post_quant_conv(z / divisor) -> Decoder -> image_postprocess(fmt).  taps: dict that receives each block's NHWC
+        output (debugging)."""
+        if self._w is None:
+            raise RuntimeError("AutoencoderKL has no weights: load_state_dict first")
+        if not z.is_cuda:
+            raise RuntimeError("AutoencoderKL (videoswap_b200) runs on CUDA only")
+        if z.dim() != 4 or z.shape[1] != self.config.latent_channels:
+            raise ValueError(f"expected latents [n, {self.config.latent_channels}, h, w], got {tuple(z.shape)}")
+        w = self._w
+
+        def tap(name, t):
+            if taps is not None:
+                taps[name] = t
+
+        z = z.contiguous() if z.dtype in (torch.float16, torch.float32) else z.float().contiguous()
+        x = ops.vae_latent_in(z, divisor, w["latent_in"])
+        x = ops.conv_in(x, *w["conv_in"])
+        tap("conv_in", x)
+        x = self._resnet(x, w["mid"][0])
+        x = self._attention(x, w["attn"])
+        tap("mid_block.attentions.0", x)
+        x = self._resnet(x, w["mid"][1])
+        tap("mid_block", x)
+        for i, blk in enumerate(w["up"]):
+            for r in blk["resnets"]:
+                x = self._resnet(x, r)
+            if blk["upsampler"] is not None:
+                x = ops.upsample_conv3x3_packed(x, *blk["upsampler"])
+            tap(f"up_blocks.{i}", x)
+        x = ops.groupnorm(x, *w["norm_out"], self._groups(), EPS, silu=True)
+        x = ops.conv3x3(x, *w["conv_out"])
+        tap("conv_out", x)
+        return ops.image_postprocess(x, fmt)
+
+    @torch.no_grad()
+    def decode(self, z: torch.Tensor, return_dict: bool = True):
+        """AutoencoderKL.decode: CUDA latents [n, 4, h, w] (fp16 / fp32) -> sample fp16 [n, 3, 8h, 8w] (not clamped)."""
+        sample = self._run(z, 1.0, ops.IMG_SAMPLE)
+        return DecoderOutput(sample=sample) if return_dict else (sample,)
+
+    @torch.no_grad()
+    def decode_postprocess(self, latents: torch.Tensor, output_type: str = "pil"):
+        """VaeImageProcessor.postprocess(decode(latents / scaling_factor)) in one pass (pipeline_videoswap.py:603-610):
+        "pt" fp32 [n, 3, H, W] in [0, 1], "np" fp32 numpy [n, H, W, 3], "pil" a list of RGB PIL images."""
+        fmt = {"pt": ops.IMG_PT, "np": ops.IMG_NP, "pil": ops.IMG_PIL}.get(output_type)
+        if fmt is None:
+            raise ValueError(f"output_type must be 'pt', 'np' or 'pil', got {output_type!r}")
+        img = self._run(latents, self.config.scaling_factor, fmt)
+        if output_type == "pt":
+            return img
+        img = img.cpu().numpy()
+        if output_type == "np":
+            return img
+        from PIL import Image
+        return [Image.fromarray(a) for a in img]
