@@ -162,7 +162,10 @@ int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0, const voi
  *   (row stride ldr; may alias `out`); mode 1 = GEGLU on packed weights (N / 2 output columns).  Folded LayerNorm of A:
  *   ln_u [N] with ln_stats [M, 2] (rstd, -mean rstd) or ln_parts [ln_nparts][M][2] (sum, sum of squares).
  *   ln_sums_out [n_tiles][M][2]: (sum, sum of squares) of the stored fp16 outputs per row and column tile of width BN.
- *   force_bn 0 = automatic column-tile width, else 64 / 128 / 160 / 256. */
+ *   force_bn 0 = automatic column-tile width, else 64 / 128 / 160 / 256.
+ *   stride2 (with taps 9): 3x3 conv with stride 2 of the input zero-padded by one column on the right and one row at the
+ *   bottom only (diffusers Downsample2D(padding=0)); H, W = the input size (both even), M = nimg (H / 2) (W / 2), output
+ *   NHWC [nimg, H / 2, W / 2, N]; A dense (lda1 = K1, K1 % 64 == 0), no A2, bias only, N % 32 == 0. */
 typedef struct vs_gemm_desc {
   const void* A; int K1; int lda1;
   const void* A2; int K2; int lda2;
@@ -181,6 +184,7 @@ typedef struct vs_gemm_desc {
   int mode;
   int force_bn;
   int OH, OW;
+  int stride2;
 } vs_gemm_desc;
 int vs_gemm_ex(void* stream, const vs_gemm_desc* desc);
 int vs_pack_conv3x3(void* stream, const void* d_w, int cout, int cin, void* d_out);
@@ -262,6 +266,28 @@ int vs_vae_latent_in(void* stream, const void* d_z, int z_is_f32, int nimg, int 
  * format 0 the sample x itself, fp16 NCHW [nimg, 3, H, W]; 1 ("pt") y fp32 NCHW; 2 ("np") y fp32 NHWC [nimg, H, W, 3];
  * 3 ("pil") uint8 NHWC round-half-even(y * 255). */
 int vs_image_postprocess(void* stream, const void* d_x, int nimg, int H, int W, int channels, int format, void* d_out);
+
+/* ---- VAE encoder (diffusers 0.19.3 AutoencoderKL.encode + DiagonalGaussianDistribution; the reference's
+ * prepare_image_latents, pipeline_videoswap.py:204-233).  The encoder is a sequence of the GEMM / conv / conv_in /
+ * GroupNorm / attention entry points above and these four. */
+/* Downsample2D(padding=0): 3x3 conv with stride 2 of NHWC d_x [nimg, H, W, C] zero-padded by one column on the right and
+ * one row at the bottom (H, W even, C % 64 == 0), as an implicit GEMM on the tensor cores (no im2col): vs_gemm_ex with
+ * taps 9 and stride2 = 1.  d_w_packed: vs_pack_conv3x3 panel [Cout, 9 C]; d_out NHWC [nimg, H / 2, W / 2, Cout]. */
+int vs_downsample_conv3x3(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w_packed, int Cout,
+                          const float* d_bias, void* d_out);
+/* Encoder entry: NHWC fp16 d_out [nimg, H, W, 4] with channel 3 zero (the input of vs_conv_in with cin = 4).  src_format
+ * 0: uint8 NHWC frames [nimg, H, W, 3], normalised as VaeImageProcessor.preprocess + the fp16 cast compute it,
+ * fl16(fl32(2 fl32(u / 255) - 1)); 1 / 2: fp16 / fp32 NCHW [nimg, 3, H, W] already in [-1, 1], rounded to fp16. */
+int vs_vae_image_in(void* stream, const void* d_x, int src_format, int nimg, int H, int W, void* d_out);
+/* Encoder exit: quant_conv (1x1, 8 -> 8) in fp32 of conv_out's NHWC fp16 d_x [nimg, h, w, 8] -> the moments
+ * (DiagonalGaussianDistribution.parameters: mean in channels 0..3, logvar in 4..7) fp16 NCHW d_out [nimg, 8, h, w].
+ * d_wb: fp32 weight [8][8] then bias [8]. */
+int vs_vae_moments(void* stream, const void* d_x, int nimg, int h, int w, const float* d_wb, void* d_out);
+/* The posterior: scale (mean + exp(0.5 clamp(logvar, -30, 20)) noise) in fp32 from the moments d_params [nimg, 8, h, w]
+ * and fp16 d_noise [nimg, 4, h, w]; d_noise NULL gives scale mean (the mode).  d_out fp16 [nimg, 4, h, w] (layout 0) or
+ * [1, 4, nimg, h, w] (layout 1: the frames of one video, as the inversion loop takes them). */
+int vs_vae_posterior(void* stream, const void* d_params, const void* d_noise, int nimg, int h, int w, float scale, int layout,
+                     void* d_out);
 
 /* ---- measurement hooks (bench.py): per-launch CUDA-event timing on the launching stream, by kernel category
  * 0 gemm, 1 conv3x3, 2 spatial/cross attention (and the VAE's row softmax), 3 temporal attention, 4 groupnorm, 5 layernorm,

@@ -55,6 +55,7 @@ class GemmDescStruct(C.Structure):
         ("mode", _I),
         ("force_bn", _I),
         ("OH", _I), ("OW", _I),
+        ("stride2", _I),
     ]
 
 _SIGNATURES = {
@@ -117,6 +118,10 @@ _SIGNATURES = {
     "vs_transpose_pad": (_I, [_P, _P, _I, _I, _I, _P]),
     "vs_vae_latent_in": (_I, [_P, _P, _I, _I, _I, _I, _F, _P, _P]),
     "vs_image_postprocess": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
+    "vs_downsample_conv3x3": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P]),
+    "vs_vae_image_in": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "vs_vae_moments": (_I, [_P, _P, _I, _I, _I, _P, _P]),
+    "vs_vae_posterior": (_I, [_P, _P, _P, _I, _I, _I, _F, _I, _P]),
 }
 
 _lib = None

@@ -58,6 +58,7 @@ extern "C" int vs_gemm_ex(void* stream, const vs_gemm_desc* d) {
   g.mode = d->mode;
   g.force_bn = d->force_bn;
   g.OH = d->OH; g.OW = d->OW;
+  g.stride2 = d->stride2;
   return gemm_tc((cudaStream_t)stream, g);
 }
 
@@ -222,6 +223,26 @@ extern "C" int vs_vae_latent_in(void* stream, const void* d_z, int z_is_f32, int
 }
 extern "C" int vs_image_postprocess(void* stream, const void* d_x, int nimg, int H, int W, int channels, int format, void* d_out) {
   return image_postprocess((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, channels, format, d_out);
+}
+extern "C" int vs_downsample_conv3x3(void* stream, const void* d_x, int nimg, int H, int W, int C, const void* d_w_packed,
+                                     int Cout, const float* d_bias, void* d_out) {
+  VS_REQUIRE(d_x && d_w_packed && d_out, "vs_downsample_conv3x3: null pointer");
+  GemmArgs g;
+  g.A = (const __half*)d_x; g.K1 = C; g.lda1 = C; g.Bw = (const __half*)d_w_packed; g.taps = 9; g.stride2 = 1;
+  g.nimg = nimg; g.H = H; g.W = W; g.M = nimg * (H / 2) * (W / 2); g.N = Cout; g.bias = d_bias; g.out = (__half*)d_out;
+  g.ldc = Cout;
+  return gemm_tc((cudaStream_t)stream, g);
+}
+extern "C" int vs_vae_image_in(void* stream, const void* d_x, int src_format, int nimg, int H, int W, void* d_out) {
+  return vae_image_in((cudaStream_t)stream, d_x, src_format, nimg, H, W, (__half*)d_out);
+}
+extern "C" int vs_vae_moments(void* stream, const void* d_x, int nimg, int h, int w, const float* d_wb, void* d_out) {
+  return vae_moments((cudaStream_t)stream, (const __half*)d_x, nimg, h, w, d_wb, (__half*)d_out);
+}
+extern "C" int vs_vae_posterior(void* stream, const void* d_params, const void* d_noise, int nimg, int h, int w, float scale,
+                                int layout, void* d_out) {
+  return vae_posterior((cudaStream_t)stream, (const __half*)d_params, (const __half*)d_noise, nimg, h, w, scale, layout,
+                       (__half*)d_out);
 }
 
 extern "C" int vs_profile_enable(int on) { prof_enable(on != 0); return 0; }

@@ -23,6 +23,8 @@
 // (column) EARLIER, so coordinate y + 1 of that view is row y of the tensor and the last row falls off the end into the
 // zero fill -- which is exactly the padding the up-sampled image has below row 2n - 2.  Only coordinates >= 1 of such a
 // view are ever read.  Output pixels beyond the target extent (parity 1 on an odd axis) are never stored.
+// A 3x3 conv with stride 2 and right / bottom padding (the VAE encoder's down-samplers) tiles the output pixels and reads
+// its taps through four parity views of the input (GemmParamsS2), so no im2col is materialised.
 //
 // Epilogue (per consumer warp, 16 rows of each 64-row half, one half after the other): registers -> [folded LayerNorm:
 // rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU -> fp16 -> warp-private
@@ -93,6 +95,16 @@ struct GemmParamsSub : GemmParams {
   int sub_short;         // bit 0 / 1: the third row / column tap of this parity reads through tmS
 };
 
+// 3x3 stride-2 conv of pad(x, (0, 1, 0, 1)) (diffusers Downsample2D(padding=0), the VAE encoder's down-samplers), its own
+// instantiations for the same reason.  The input is read through four parity views of the NHWC tensor: view (py, px)
+// starts at pixel (py, px) and has doubled pixel strides and dims (W / 2, H / 2), so its element (x', y') is input pixel
+// (2 x' + px, 2 y' + py).  tmA is view (0, 0), tmP[k - 1] view k = 2 py + px.  Tap (dy, dx) in {0, 1, 2}^2 of output
+// pixel (x, y) reads view (dy & 1, dx & 1) at (x + (dx >> 1), y + (dy >> 1)); at the last output column / row an offset
+// of 1 lands on x' = W / 2 (y' = H / 2), outside the view, and the TMA zero fill is exactly the right / bottom padding.
+struct GemmParamsS2 : GemmParams {
+  CUtensorMap tmP[3];
+};
+
 template <int BN>
 struct Cfg {
   // Cooperative (both consumers on one 128 x BN tile, 64 rows each) for BN = 256: 128 accumulators a thread.  Ping-pong
@@ -117,6 +129,7 @@ template <int BN, int EPI, typename Params>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ Params p) {
   using C = Cfg<BN>;
   constexpr bool SUB = std::is_same<Params, GemmParamsSub>::value;
+  constexpr bool S2 = std::is_same<Params, GemmParamsS2>::value;
   constexpr bool GEGLU = (EPI & EPI_F_GEGLU) != 0, HAS_RES = (EPI & EPI_F_RES) != 0, HAS_RV = (EPI & EPI_F_RV) != 0;
   // LN: the A operand is the RAW input of a LayerNorm whose affine map is folded into the weights:
   //   LN(x) W^T = rstd (x W'^T) - rstd mean u + c,  W' = W * gamma, u[n] = sum_k W'[n,k], c = beta W^T + bias (the `bias`)
@@ -150,6 +163,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       if (p.sub_short & 1) prefetch_tmap(&p.tmS[0]);
       if (p.sub_short & 2) prefetch_tmap(&p.tmS[1]);
       if (p.sub_short == 3) prefetch_tmap(&p.tmS[2]);
+    }
+    if constexpr (S2) {
+      for (int k = 0; k < 3; ++k) prefetch_tmap(&p.tmP[k]);
     }
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
@@ -195,9 +211,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
             const bool sy = short_y && dy == p.tap_y0 + 2, sx = short_x && dx == tap_x0 + 2;   // third tap of an odd axis
             if (sy || sx) tm = sy ? (sx ? &p.tmS[2] : &p.tmS[0]) : &p.tmS[1];
           }
+          int ox = dx, oy = dy;                // tap offset in the coordinates of the view `tm`
+          if constexpr (S2) {                  // parity view of the tap, offset 0 or 1 inside it
+            const int par = ((dy & 1) << 1) | (dx & 1);
+            if (par) tm = &p.tmP[par - 1];
+            ox = dx >> 1; oy = dy >> 1;
+          }
           const int c = (first ? r : r - kb_src1) * BK;
           mbar_expect_tx(fb, C::STAGE_BYTES);
-          if (conv) tma_load_4d(a_dst, tm, fb, c, x0 + dx, y0 + dy, i0);
+          if (conv) tma_load_4d(a_dst, tm, fb, c, x0 + ox, y0 + oy, i0);
           else tma_load_2d(a_dst, tm, fb, c, m0);
           tma_load_2d(a_dst + A_STAGE_BYTES, &p.tmB, fb, kcoord, n0);
         }
@@ -534,6 +556,8 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   GemmParamsSub ps;                            // the GemmParams part is what every launch but an odd-sized sub-pixel one takes
   memset(&ps, 0, sizeof(ps));
   GemmParams& p = ps;
+  GemmParamsS2 p2;                             // stride 2: the parity views; its GemmParams part is copied from p at launch
+  memset(&p2, 0, sizeof(p2));
   // sub-pixel conv: output extent OH x OW (2H or 2H - 1 rows, 2W or 2W - 1 columns); parity 0 of an odd axis has 3 taps
   const bool sub = a.taps == 4;
   const int OH = sub && a.OH > 0 ? a.OH : 2 * a.H, OW = sub && a.OW > 0 ? a.OW : 2 * a.W;
@@ -570,28 +594,42 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   p.ldc = a.ldc;
   p.stages = get_option("gemm_stages");
 
+  // stride 2 (GemmParamsS2): the tiles walk the (H / 2) x (W / 2) output pixels; every other conv tiles its input grid
+  const bool s2 = a.stride2 != 0;
+  if (s2) VS_REQUIRE(a.taps == 9 && !two && a.H % 2 == 0 && a.W % 2 == 0 && a.lda1 == a.K1 && a.mode == EPI_LINEAR &&
+                     !a.ln_stats && !a.ln_parts,
+                     "gemm_tc: the stride-2 conv takes one dense NHWC source of even height and width (got %dx%d)", a.H, a.W);
+  const int GH = s2 ? a.H / 2 : a.H, GW = s2 ? a.W / 2 : a.W;
   if (a.taps != 1) {
-    VS_REQUIRE(a.nimg > 0 && a.H > 0 && a.W > 0 && a.M == a.nimg * a.H * a.W, "gemm_tc: bad conv geometry");
+    VS_REQUIRE(a.nimg > 0 && GH > 0 && GW > 0 && a.M == a.nimg * GH * GW, "gemm_tc: bad conv geometry");
     p.a_rank = 4;
     // 3x3: taps (-1..1)^2.  Sub-pixel (one output parity (py, px) of nearest up-sampling + 3x3, see pack_conv_subpixel):
     // taps {py - 1, py} x {px - 1, px}, output pixel (2 y + py, 2 x + px) of the OH x OW image; on an odd axis parity 0
-    // has the taps {-1, 0, 0'} with 0' read through the shifted view (tmS).
-    if (a.taps == 9) { p.tap_x0 = p.tap_y0 = -1; p.tap_w = 3; p.osy = p.osx = 1; p.ooy = p.oox = 0; p.OH = a.H; p.OW = a.W; }
+    // has the taps {-1, 0, 0'} with 0' read through the shifted view (tmS).  Stride 2: taps (0..2)^2 on the parity views.
+    if (s2) { p.tap_x0 = p.tap_y0 = 0; p.tap_w = 3; p.osy = p.osx = 1; p.ooy = p.oox = 0; p.OH = GH; p.OW = GW; }
+    else if (a.taps == 9) { p.tap_x0 = p.tap_y0 = -1; p.tap_w = 3; p.osy = p.osx = 1; p.ooy = p.oox = 0; p.OH = a.H; p.OW = a.W; }
     else {
       VS_REQUIRE((a.sub_py | 1) == 1 && (a.sub_px | 1) == 1, "gemm_tc: sub-pixel parity must be 0 or 1");
       p.tap_y0 = a.sub_py - 1; p.tap_x0 = a.sub_px - 1; p.tap_w = sub_tx;
       ps.sub_short = (sub_ty == 3 ? 1 : 0) | (sub_tx == 3 ? 2 : 0);
       p.osy = p.osx = 2; p.ooy = a.sub_py; p.oox = a.sub_px; p.OH = OH; p.OW = OW;
     }
-    const ConvTile t = pick_conv_tile(a.nimg, a.H, a.W);
-    p.nimg = a.nimg; p.H = a.H; p.W = a.W; p.TW = t.tw; p.TH = t.th; p.TN = t.tn;
+    const ConvTile t = pick_conv_tile(a.nimg, GH, GW);
+    p.nimg = a.nimg; p.H = GH; p.W = GW; p.TW = t.tw; p.TH = t.th; p.TN = t.tn;
     p.tw_log = ilog2(t.tw);
     p.thw_log = ilog2(t.tw * t.th);
-    p.tiles_x = (a.W + t.tw - 1) / t.tw;
-    p.tiles_y = (a.H + t.th - 1) / t.th;
+    p.tiles_x = (GW + t.tw - 1) / t.tw;
+    p.tiles_y = (GH + t.th - 1) / t.th;
     p.m_tiles = p.tiles_x * p.tiles_y * ((a.nimg + t.tn - 1) / t.tn);
     const uint32_t box[4] = {BK, (uint32_t)t.tw, (uint32_t)t.th, (uint32_t)t.tn};
-    {
+    if (s2) {
+      // parity view k = 2 py + px: starts at input pixel (px, py), (W / 2) x (H / 2) pixels at twice the pixel strides
+      const uint64_t dims[4] = {(uint64_t)a.K1, (uint64_t)GW, (uint64_t)GH, (uint64_t)a.nimg};
+      const uint64_t str[3] = {(uint64_t)a.K1 * 4, (uint64_t)a.K1 * 4 * a.W, (uint64_t)a.K1 * 2 * a.W * a.H};
+      if (make_tmap_f16(&p.tmA, a.A, 4, dims, str, box, 1)) return 3;
+      for (int k = 1; k < 4; ++k)
+        if (make_tmap_f16(&p2.tmP[k - 1], a.A + ((long long)(k >> 1) * a.W + (k & 1)) * a.K1, 4, dims, str, box, 1)) return 3;
+    } else {
       const uint64_t dims[4] = {(uint64_t)a.K1, (uint64_t)a.W, (uint64_t)a.H, (uint64_t)a.nimg};
       const uint64_t str[3] = {(uint64_t)a.lda1 * 2, (uint64_t)a.lda1 * 2 * a.W, (uint64_t)a.lda1 * 2 * a.W * a.H};
       if (make_tmap_f16(&p.tmA, a.A, 4, dims, str, box, 1)) return 3;
@@ -654,6 +692,17 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   if (a.mode == EPI_GEGLU) {
     if (p.ln_stats || p.ln_parts) return launch<256, EPI_F_GEGLU | EPI_F_LN>(st, p);
     return launch<256, EPI_F_GEGLU>(st, p);
+  }
+  if (s2) {
+    VS_REQUIRE(a.residual == nullptr && a.rowvec == nullptr && a.ln_sums_out == nullptr && p.staged,
+               "gemm_tc: the stride-2 conv takes a bias only and needs N %% 32 == 0");
+    static_cast<GemmParams&>(p2) = p;
+    switch (bn) {
+      case 64: return launch<64, 0, GemmParamsS2>(st, p2);
+      case 128: return launch<128, 0, GemmParamsS2>(st, p2);
+      case 256: return launch<256, 0, GemmParamsS2>(st, p2);
+      default: return launch<160, 0, GemmParamsS2>(st, p2);
+    }
   }
   if (sub && ((OH | OW) & 1)) {
     VS_REQUIRE(a.residual == nullptr && a.rowvec == nullptr && p.staged, "gemm_tc: an odd-sized sub-pixel conv takes a bias only");

@@ -44,6 +44,9 @@ struct GemmArgs {
   // taps == 4: output extent, 2H or 2H - 1 rows and 2W or 2W - 1 columns (0 = 2H / 2W).  Along an odd axis parity 0 has
   // 3 taps, so Bw holds 2x3, 3x2 or 3x3 taps (the panels pack_conv_subpixel / pack_conv3x3 make, see upsample_conv3x3).
   int OH = 0, OW = 0;
+  // taps == 9 with stride2 != 0: 3x3 conv with stride 2 of pad(A, (0, 1, 0, 1)) (right / bottom zero padding, diffusers
+  // Downsample2D(padding=0)); H, W = the input size (even), M = nimg (H / 2) (W / 2), one dense source, bias only.
+  int stride2 = 0;
 };
 int gemm_tc(cudaStream_t st, const GemmArgs& a);
 int gemm_n_tiles(const GemmArgs& a);         // column tiles gemm_tc will use (taps == 1)
@@ -119,6 +122,17 @@ int vae_latent_in(cudaStream_t st, const void* z, int z_is_f32, int nimg, int h,
 // VAE decoder exit: channels 0..2 of NHWC fp16 x [nimg, H, W, cs] (cs % 8 == 0) in one of the formats below.
 enum ImageFormat { IMG_SAMPLE = 0, IMG_PT = 1, IMG_NP = 2, IMG_PIL = 3 };
 int image_postprocess(cudaStream_t st, const __half* x, int nimg, int H, int W, int cs, int format, void* out);
+// VAE encoder entry: images -> NHWC fp16 [nimg, H, W, 4] with channel 3 zero.  uint8 NHWC frames [nimg, H, W, 3] are
+// normalised as VaeImageProcessor.preprocess does (2 (u / 255) - 1); float NCHW [nimg, 3, H, W] are taken as they are.
+enum VaeImageSource { VAE_IN_U8_NHWC = 0, VAE_IN_F16_NCHW = 1, VAE_IN_F32_NCHW = 2 };
+int vae_image_in(cudaStream_t st, const void* x, int src, int nimg, int H, int W, __half* out);
+// VAE encoder exit: quant_conv of conv_out's NHWC fp16 [nimg, h, w, 8] in fp32 -> moments fp16 NCHW [nimg, 8, h, w];
+// wb fp32 = weight [8][8] then bias [8].
+int vae_moments(cudaStream_t st, const __half* x, int nimg, int h, int w, const float* wb, __half* out);
+// scale (mean + exp(0.5 clamp(logvar, -30, 20)) noise) (noise fp16 [nimg, 4, h, w], or null: scale mean) from the moments,
+// fp16 [nimg, 4, h, w] (layout 0) or [1, 4, nimg, h, w] (layout 1).
+int vae_posterior(cudaStream_t st, const __half* params, const __half* noise, int nimg, int h, int w, float scale, int layout,
+                  __half* out);
 // eps = u + s (c - u); x_prev = sqrt(a_p) (x - sqrt(1-a_t) eps)/sqrt(a_t) + sqrt(1-a_p) eps.  eps2: [2, n] (uncond
 // first) or [1, n] when guidance is disabled (cfg == 0).
 int cfg_ddim_step(cudaStream_t st, const void* eps2, const void* latents, int is_f32, size_t n, int cfg,

@@ -527,6 +527,78 @@ __global__ void image_postprocess_kernel(const __half* __restrict__ x, long long
   }
 }
 
+// ---------------------------------------------------------------------------------------------- VAE encoder entry / exit
+// Encoder input as NHWC fp16 [n, H, W, 4] with channel 3 zero (so the tensor-core conv_in, ci = 4, runs the 3 -> 128 conv).
+// uint8 NHWC frames [n, H, W, 3]: what VaeImageProcessor.preprocess and the fp16 cast of prepare_image_latents compute,
+// fl16(fl32(2 fl32(u / 255) - 1)) -- numpy's float32 division, 2 y exact, the subtraction rounded on its own (no FMA).
+__global__ void vae_image_in_u8_kernel(const uint8_t* __restrict__ x, long long npix, __half* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
+    __half o[4];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float y = __fdiv_rn((float)x[i * 3 + c], 255.f);
+      o[c] = __float2half_rn(__fsub_rn(__fmul_rn(2.f, y), 1.f));
+    }
+    o[3] = __float2half_rn(0.f);
+    *reinterpret_cast<uint2*>(out + i * 4) = *reinterpret_cast<const uint2*>(o);
+  }
+}
+
+// float NCHW images [n, 3, H, W] (fp16, or fp32 rounded to fp16 once), already in [-1, 1] (AutoencoderKL.encode's input)
+template <typename T>
+__global__ void vae_image_in_nchw_kernel(const T* __restrict__ x, long long npix, int hw, __half* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
+    const long long img = i / hw, p = i % hw;
+    __half o[4];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = __float2half_rn((float)x[(img * 3 + c) * hw + p]);
+    o[3] = __float2half_rn(0.f);
+    *reinterpret_cast<uint2*>(out + i * 4) = *reinterpret_cast<const uint2*>(o);
+  }
+}
+
+// quant_conv (1x1, 8 -> 8) of conv_out's NHWC fp16 output [n, h, w, 8] in fp32, written as diffusers' `parameters`
+// (the moments: mean in channels 0..3, logvar in 4..7) fp16 NCHW [n, 8, h, w].  wb: fp32 [8][8] weight then [8] bias.
+// Fixed order, no contraction: out_c = ((b_c + w_c0 x_0) + w_c1 x_1) + ... + w_c7 x_7.
+__global__ void vae_moments_kernel(const __half* __restrict__ x, long long npix, int hw, const float* __restrict__ wb,
+                                   __half* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = *reinterpret_cast<const uint4*>(x + i * 8);
+    const __half* h = reinterpret_cast<const __half*>(&v);
+    float xs[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) xs[k] = __half2float(h[k]);
+    const long long img = i / hw, p = i % hw;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      float acc = wb[64 + c];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc = __fadd_rn(acc, __fmul_rn(wb[c * 8 + k], xs[k]));
+      out[(img * 8 + c) * hw + p] = __float2half_rn(acc);
+    }
+  }
+}
+
+// DiagonalGaussianDistribution: scale (mean + exp(0.5 clamp(logvar, -30, 20)) noise) in fp32 from the fp16 parameters
+// [n, 8, h, w] and fp16 noise [n, 4, h, w]; without noise scale mean (the mode).  Output fp16 [n, 4, h, w] (layout 0) or
+// [1, 4, n, h, w] (layout 1, the frames of one video as the inversion loop takes them).
+__global__ void vae_posterior_kernel(const __half* __restrict__ prm, const __half* __restrict__ noise, int nimg, int hw,
+                                     float scale, int layout, __half* __restrict__ out) {
+  const long long total = (long long)nimg * 4 * hw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long img = i / (4LL * hw), r = i % (4LL * hw);
+    const int c = (int)(r / hw);
+    const long long p = r % hw;
+    float v = __half2float(prm[(img * 8 + c) * hw + p]);
+    if (noise != nullptr) {
+      const float lv = fminf(fmaxf(__half2float(prm[(img * 8 + 4 + c) * hw + p]), -30.f), 20.f);
+      v = __fadd_rn(v, __fmul_rn(expf(__fmul_rn(0.5f, lv)), __half2float(noise[i])));
+    }
+    const long long o = layout ? ((long long)c * nimg + img) * hw + p : i;
+    out[o] = __float2half_rn(__fmul_rn(scale, v));
+  }
+}
+
 inline unsigned capped(size_t n) {
   size_t b = (n + TPB - 1) / TPB;
   const size_t cap = (size_t)num_sms() * 16;
@@ -713,6 +785,35 @@ int image_postprocess(cudaStream_t st, const __half* x, int nimg, int H, int W, 
   const int out_bytes = format == IMG_PIL ? 3 : (format == IMG_SAMPLE ? 6 : 12);
   ProfScope prof(st, PC_OTHER, (double)npix * (16 + out_bytes));
   image_postprocess_kernel<<<capped((size_t)npix), TPB, 0, st>>>(x, npix, H * W, cs, format, out);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+int vae_image_in(cudaStream_t st, const void* x, int src, int nimg, int H, int W, __half* out) {
+  VS_REQUIRE(x && out && nimg > 0 && H > 0 && W > 0, "vae_image_in: bad arguments");
+  VS_REQUIRE(src >= VAE_IN_U8_NHWC && src <= VAE_IN_F32_NCHW, "vae_image_in: unknown source format %d", src);
+  const long long npix = (long long)nimg * H * W;
+  const int in_bytes = src == VAE_IN_U8_NHWC ? 3 : (src == VAE_IN_F16_NCHW ? 6 : 12);
+  ProfScope prof(st, PC_OTHER, (double)npix * (in_bytes + 8));   // bytes read + written
+  if (src == VAE_IN_U8_NHWC) vae_image_in_u8_kernel<<<capped((size_t)npix), TPB, 0, st>>>((const uint8_t*)x, npix, out);
+  else if (src == VAE_IN_F16_NCHW) vae_image_in_nchw_kernel<__half><<<capped((size_t)npix), TPB, 0, st>>>((const __half*)x, npix, H * W, out);
+  else vae_image_in_nchw_kernel<float><<<capped((size_t)npix), TPB, 0, st>>>((const float*)x, npix, H * W, out);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+int vae_moments(cudaStream_t st, const __half* x, int nimg, int h, int w, const float* wb, __half* out) {
+  VS_REQUIRE(x && wb && out && nimg > 0 && h > 0 && w > 0, "vae_moments: bad arguments");
+  const long long npix = (long long)nimg * h * w;
+  ProfScope prof(st, PC_OTHER, (double)npix * 32);   // 16 bytes read + 16 written per pixel
+  vae_moments_kernel<<<capped((size_t)npix), TPB, 0, st>>>(x, npix, h * w, wb, out);
+  VS_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+int vae_posterior(cudaStream_t st, const __half* params, const __half* noise, int nimg, int h, int w, float scale, int layout,
+                  __half* out) {
+  VS_REQUIRE(params && out && nimg > 0 && h > 0 && w > 0 && (layout | 1) == 1, "vae_posterior: bad arguments");
+  const long long n = (long long)nimg * 4 * h * w;
+  ProfScope prof(st, PC_OTHER, (double)n * (noise ? 8 : 4));   // bytes read + written
+  vae_posterior_kernel<<<capped((size_t)n), TPB, 0, st>>>(params, noise, nimg, h * w, scale, layout, out);
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

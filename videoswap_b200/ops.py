@@ -380,6 +380,61 @@ def image_postprocess(x, fmt):
     return out
 
 
+def downsample_conv3x3(x, w_packed, bias=None):
+    """Downsample2D(padding=0): conv3x3 with stride 2 of x zero-padded by one column on the right and one row at the
+    bottom, x [N, H, W, C] (H, W even, C % 64 == 0), w_packed pack_conv3x3 [Co, 9 C] -> [N, H / 2, W / 2, Co]."""
+    _chk16(x, w_packed)
+    _chk32(bias)
+    n, H, W, Ci = x.shape
+    co = w_packed.shape[0]
+    assert w_packed.shape[1] == 9 * Ci, "expected a pack_conv3x3 panel"
+    out = torch.empty((n, H // 2, W // 2, co), dtype=torch.float16, device=x.device)
+    _lib.call("vs_downsample_conv3x3", _stream(), _p(x), n, H, W, Ci, _p(w_packed), co, _p(bias), _p(out))
+    return out
+
+
+VAE_IN_U8_NHWC, VAE_IN_F16_NCHW, VAE_IN_F32_NCHW = 0, 1, 2
+
+
+def vae_image_in(x):
+    """Encoder input -> NHWC fp16 [n, H, W, 4] with channel 3 zero.  x: uint8 frames [n, H, W, 3] (normalised as
+    VaeImageProcessor.preprocess does, 2 (u / 255) - 1) or fp16 / fp32 images [n, 3, H, W] in [-1, 1] (rounded to fp16)."""
+    assert x.is_cuda and x.is_contiguous() and x.dim() == 4, "expected a contiguous 4-D CUDA tensor"
+    if x.dtype == torch.uint8:
+        assert x.shape[3] == 3, "uint8 frames are [n, H, W, 3]"
+        src, (n, H, W) = VAE_IN_U8_NHWC, x.shape[:3]
+    else:
+        assert x.dtype in (torch.float16, torch.float32) and x.shape[1] == 3, "float images are [n, 3, H, W] fp16 / fp32"
+        src = VAE_IN_F16_NCHW if x.dtype == torch.float16 else VAE_IN_F32_NCHW
+        n, _, H, W = x.shape
+    out = torch.empty((n, H, W, 4), dtype=torch.float16, device=x.device)
+    _lib.call("vs_vae_image_in", _stream(), _p(x), src, n, H, W, _p(out))
+    return out
+
+
+def vae_moments(x, wb):
+    """quant_conv in fp32: conv_out's x [n, h, w, 8] fp16, wb fp32 [72] (weight [8, 8], then bias [8]) -> the moments
+    fp16 NCHW [n, 8, h, w] (mean, then logvar)."""
+    _chk16(x)
+    _chk32(wb)
+    n, h, w, Cc = x.shape
+    assert Cc == 8 and wb.numel() == 72
+    out = torch.empty((n, 8, h, w), dtype=torch.float16, device=x.device)
+    _lib.call("vs_vae_moments", _stream(), _p(x), n, h, w, _p(wb), _p(out))
+    return out
+
+
+def vae_posterior(params, noise=None, scale=1.0, video=False):
+    """scale (mean + exp(0.5 clamp(logvar, -30, 20)) noise) from the moments params [n, 8, h, w] fp16 and noise
+    [n, 4, h, w] fp16 (None: scale mean).  Output fp16 [n, 4, h, w], or with video=True [1, 4, n, h, w]."""
+    _chk16(params, noise)
+    n, c8, h, w = params.shape
+    assert c8 == 8 and (noise is None or tuple(noise.shape) == (n, 4, h, w))
+    out = torch.empty((1, 4, n, h, w) if video else (n, 4, h, w), dtype=torch.float16, device=params.device)
+    _lib.call("vs_vae_posterior", _stream(), _p(params), _p(noise), n, h, w, float(scale), int(video), _p(out))
+    return out
+
+
 def temporal_attention(qkv, heads):
     """qkv [B, F, HW, 3C] -> [B, F, HW, C]: attention over the F axis for every (b, pixel, head)."""
     _chk16(qkv)

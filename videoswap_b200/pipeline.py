@@ -2,9 +2,10 @@
 denoising part of `VideoSwapPipeline` (videoswap/pipelines/pipeline_videoswap.py:427-619 `__call__`, :622-721 `invert`).
 
 Scope (SURVEY.md 8): the loop body -- CFG batch duplication, UNet forward, CFG combine, scheduler step, adapter
-residual window -- runs on the native kernels.  Text encoding (CLIP), VAE encode and prompt/LoRA handling are callers on
-either side of this path (8f) and are NOT part of this package: the pipeline takes `prompt_embeds` / `latents` tensors and
-returns latents, or, given a `vae` (videoswap_b200.vae.AutoencoderKL), the decoded frames.
+residual window -- runs on the native kernels.  Text encoding (CLIP) and prompt/LoRA handling are callers on either side
+of this path (8f) and are NOT part of this package: the pipeline takes `prompt_embeds` and `latents` tensors and returns
+latents.  Given a `vae` (videoswap_b200.vae.AutoencoderKL) it also encodes the source frames for the DDIM inversion
+(`prepare_image_latents`, `invert(video=...)`) and decodes the result into frames.
 """
 from __future__ import annotations
 
@@ -92,14 +93,37 @@ def _combine(eps, latents, guidance_scale, a_t, a_p, cfg):
     return ops.cfg_ddim_step(eps, latents, guidance_scale, a_t, a_p, cfg=cfg)
 
 
+def _frames_to_uint8(frames) -> torch.Tensor:
+    """The PIL half of VaeImageProcessor.preprocess (diffusers 0.19.3 image_processor.py, vae_scale_factor 8, resample
+    "lanczos"): each frame resized to the next lower multiple of 8 when its size is not one, then stacked as uint8
+    [F, H, W, 3] for one upload.  The division by 255 and the normalisation run on the device (vae_image_in)."""
+    import numpy as np
+    from PIL import Image
+    if isinstance(frames, Image.Image):
+        frames = [frames]
+    if not isinstance(frames, (list, tuple)) or not frames or not all(isinstance(f, Image.Image) for f in frames):
+        raise ValueError("video must be a list of PIL images, a [F, 3, H, W] tensor or [F, 4, h, w] latents")
+    arrs = []
+    for f in frames:
+        if f.mode != "RGB":
+            raise ValueError(f"video frames must be RGB PIL images, got mode {f.mode!r}")
+        w, h = (x - x % 8 for x in f.size)
+        if (w, h) != f.size:
+            f = f.resize((w, h), resample=Image.LANCZOS)
+        arrs.append(np.asarray(f, dtype=np.uint8))
+    if len({a.shape for a in arrs}) != 1:
+        raise ValueError(f"video frames differ in size: {sorted({a.shape[:2] for a in arrs})}")
+    return torch.from_numpy(np.stack(arrs))
+
+
 class VideoSwapPipeline:
     """The denoising loop of the reference pipeline on the native path.  BASELINE.json's `TuneAVideoPipeline` alias."""
 
     def __init__(self, unet: AnimateDiffUNet3DModel, scheduler: Optional[DDIMScheduler] = None,
                  adapter: Optional[SparsePointAdapter] = None, inverse_scheduler: Optional[DDIMInverseScheduler] = None,
                  vae: Optional[AutoencoderKL] = None):
-        """vae: the decoder that turns the final latents into frames (output_type "pt" / "np" / "pil"); without it the
-        pipeline returns latents only."""
+        """vae: encodes the source video for the inversion (invert(video=...)) and turns the final latents into frames
+        (output_type "pt" / "np" / "pil"); without it the pipeline takes and returns latents only."""
         self.unet = unet
         self.scheduler = scheduler or DDIMScheduler()
         self.inverse_scheduler = inverse_scheduler or DDIMInverseScheduler()
@@ -222,10 +246,39 @@ class VideoSwapPipeline:
         return self.vae.decode_postprocess(latents, output_type)
 
     @torch.no_grad()
-    def invert(self, prompt_embeds: torch.Tensor, latents: torch.Tensor, num_inference_steps: int = 50,
-               return_dict: bool = True, controller=None, max_iters: Optional[int] = None):
+    def prepare_image_latents(self, video, generator=None) -> torch.Tensor:
+        """VaeImageProcessor.preprocess + prepare_image_latents (pipeline_videoswap.py:204-233, 660-664): the source video
+        -> fp16 latents [1, 4, F, h, w] = scaling_factor * vae.encode(frames).latent_dist.sample(generator).  video:
+          * a list of RGB PIL frames (all of one size); a size that is not a multiple of 8 is resized down to one with
+            LANCZOS, as preprocess does; the frames go to the device as one uint8 [F, H, W, 3] upload;
+          * a [F, 3, H, W] tensor in [-1, 1] (H, W multiples of 8);
+          * latents [F, 4, h, w], passed through unscaled as the reference passes them.
+        generator: a torch.Generator (CPU or CUDA) or one per frame; the noise is the reference's draw for that seed."""
+        if self.vae is None:
+            raise ValueError("encoding a video needs a VideoSwapPipeline(..., vae=AutoencoderKL)")
+        dev = self.vae.device
+        if isinstance(video, torch.Tensor):
+            if video.dim() != 4 or video.shape[1] not in (3, 4):
+                raise ValueError(f"expected a video tensor [F, 3, H, W] or latents [F, 4, h, w], got {tuple(video.shape)}")
+            if video.shape[1] == 4:
+                lat = video.to(device=dev, dtype=torch.float16)
+                return lat.permute(1, 0, 2, 3).unsqueeze(0).contiguous()
+            dist = self.vae.encode(video.to(dev).contiguous()).latent_dist
+        else:
+            frames = _frames_to_uint8(video)
+            dist = self.vae.encode_frames(frames.to(dev))
+        return dist.sample(generator, scale=self.vae.config.scaling_factor, video=True)
+
+    @torch.no_grad()
+    def invert(self, prompt_embeds: torch.Tensor, latents: Optional[torch.Tensor] = None, num_inference_steps: int = 50,
+               return_dict: bool = True, controller=None, max_iters: Optional[int] = None, *, video=None, generator=None):
         """DDIM inversion loop (pipeline_videoswap.py:677-703), guidance_scale = 1 (no CFG).  The UNet is evaluated at
-        the inverse scheduler's timestep; which noise levels the step connects is the scheduler's `convention`."""
+        the inverse scheduler's timestep; which noise levels the step connects is the scheduler's `convention`.
+        Exactly one of `latents` ([1, 4, F, h, w]) and `video` (see prepare_image_latents, with `generator`) is given."""
+        if (latents is None) == (video is None):
+            raise ValueError("invert takes exactly one of `latents` and `video`")
+        if video is not None:
+            latents = self.prepare_image_latents(video, generator)
         self.inverse_scheduler.set_timesteps(num_inference_steps)
         latents = latents.contiguous()
         for i, t in enumerate(self.inverse_scheduler.timesteps):

@@ -245,6 +245,38 @@ def vae_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...]]":
     return sh
 
 
+def vae_encoder_param_shapes(cfg: VAEConfig) -> "OrderedDict[str, Tuple[int, ...]]":
+    """Encoder-side AutoencoderKL state_dict (diffusers 0.19.3 names): Encoder (conv_in, DownEncoderBlock2D x 4 of
+    layers_per_block resnets with a stride-2 Downsample2D on all but the last, UNetMidBlock2D, conv_norm_out, conv_out to
+    2 x latent_channels with double_z) and quant_conv."""
+    sh: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    lc, boc = cfg.latent_channels, list(cfg.block_out_channels)
+    sh["encoder.conv_in.weight"] = (boc[0], cfg.in_channels, 3, 3)
+    sh["encoder.conv_in.bias"] = (boc[0],)
+    prev = boc[0]
+    for i, out in enumerate(boc):
+        for j in range(cfg.layers_per_block):
+            _vae_resnet(sh, f"encoder.down_blocks.{i}.resnets.{j}", prev if j == 0 else out, out)
+        if i < len(boc) - 1:
+            sh[f"encoder.down_blocks.{i}.downsamplers.0.conv.weight"] = (out, out, 3, 3)
+            sh[f"encoder.down_blocks.{i}.downsamplers.0.conv.bias"] = (out,)
+        prev = out
+    c = boc[-1]
+    _vae_resnet(sh, "encoder.mid_block.resnets.0", c, c)
+    a = "encoder.mid_block.attentions.0"
+    _norm(sh, a + ".group_norm", c)
+    for n in ("to_q", "to_k", "to_v", "to_out.0"):
+        sh[f"{a}.{n}.weight"] = (c, c)
+        sh[f"{a}.{n}.bias"] = (c,)
+    _vae_resnet(sh, "encoder.mid_block.resnets.1", c, c)
+    _norm(sh, "encoder.conv_norm_out", c)
+    sh["encoder.conv_out.weight"] = (2 * lc, c, 3, 3)
+    sh["encoder.conv_out.bias"] = (2 * lc,)
+    sh["quant_conv.weight"] = (2 * lc, 2 * lc, 1, 1)
+    sh["quant_conv.bias"] = (2 * lc,)
+    return sh
+
+
 def adapter_param_shapes(embedding_channels=1280, channels=(320, 640, 1280, 1280), mid_dim=128):
     """SparsePointAdapter state_dict (videoswap/models/adapter_model.py:50-70 of the reference)."""
     sh = OrderedDict()

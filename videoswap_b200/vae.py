@@ -1,11 +1,13 @@
-"""The decoder half of diffusers 0.19.3 `AutoencoderKL` (SD-1.5's VAE) on the native kernels, with the decoder-side
-config and state_dict names of diffusers.  The reference's loop ends with `vae.decode(latents / scaling_factor)` and
-`VaeImageProcessor.postprocess` (videoswap/pipelines/pipeline_videoswap.py:603-610); `decode_postprocess` replaces the two
-calls, `decode` the first.
+"""diffusers 0.19.3 `AutoencoderKL` (SD-1.5's VAE) on the native kernels, with diffusers' config and state_dict names.
+Decoder: the reference's loop ends with `vae.decode(latents / scaling_factor)` and `VaeImageProcessor.postprocess`
+(videoswap/pipelines/pipeline_videoswap.py:603-610); `decode_postprocess` replaces the two calls, `decode` the first.
+Encoder: `prepare_image_latents` starts the edit with `vae.encode(image).latent_dist.sample(generator) * scaling_factor`
+(pipeline_videoswap.py:204-233); `encode` returns the same `AutoencoderKLOutput(latent_dist=DiagonalGaussianDistribution)`.
 
 Executor: a short sequence over `ops`, activations NHWC fp16, every frame of a call in one pass (the GroupNorms are per
 image, so frames stay independent).  The mid block's single-head attention (d = 512) runs per frame as GEMMs around a row
-softmax: S = Q K^T into one [hw, hw_pad] buffer, P = softmax(S / sqrt(512)) in place, O = P V with V transposed."""
+softmax: S = Q K^T into one [hw, hw_pad] buffer, P = softmax(S / sqrt(512)) in place, O = P V with V transposed.  The
+encoder's stride-2 down-samplers run as implicit GEMMs on parity views of their input (ops.downsample_conv3x3)."""
 from __future__ import annotations
 
 import json
@@ -17,7 +19,7 @@ from typing import Dict, Optional
 import torch
 
 from . import ops
-from .spec import VAEConfig, vae_param_shapes
+from .spec import VAEConfig, vae_encoder_param_shapes, vae_param_shapes
 from .weights import seeded_state_dict
 
 EPS = 1e-6                     # resnet_eps of the SD-1.5 decoder (GroupNorms of resnets, attention and conv_norm_out)
@@ -64,6 +66,102 @@ def convert_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str,
     return out
 
 
+def _encoder_entries(sd: Dict[str, torch.Tensor], cfg: VAEConfig):
+    """The encoder / quant_conv keys of sd renamed and reshaped to vae_encoder_param_shapes(cfg) -> (dict, missing keys).
+    Decoder keys are skipped; an unknown encoder key, a key given twice or a wrong shape raises."""
+    shapes = vae_encoder_param_shapes(cfg)
+    out = {}
+    for k, v in sd.items():
+        if not k.startswith(_IGNORED_PREFIXES):
+            continue
+        name = k
+        head, _, leaf = k.rpartition(".")
+        attn, _, old = head.rpartition(".")
+        if attn == "encoder.mid_block.attentions.0" and old in _OLD_ATTN:
+            name = f"{attn}.{_OLD_ATTN[old]}.{leaf}"
+        if name not in shapes:
+            raise KeyError(f"unexpected key in the VAE state_dict: {k}")
+        if name in out:
+            raise KeyError(f"{k}: {name} is given twice (old and new attention names)")
+        want = shapes[name]
+        if tuple(v.shape) != want:
+            if name.startswith(attn + ".") and len(want) == 2 and tuple(v.shape) == want + (1, 1):
+                v = v.reshape(want)
+            else:
+                raise ValueError(f"{k}: shape {tuple(v.shape)}, expected {want}")
+        out[name] = v
+    return out, [k for k in shapes if k not in out]
+
+
+def _missing_text(missing) -> str:
+    return f"{missing[:5]}{' ...' if len(missing) > 5 else ''} ({len(missing)} keys)"
+
+
+def convert_encoder_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str, torch.Tensor]:
+    """A full AutoencoderKL state_dict -> the encoder / quant_conv keys of vae_encoder_param_shapes(cfg), in their shapes.
+    The same old attention names as convert_state_dict are renamed (encoder.mid_block.attentions.0); decoder keys are
+    skipped; an unknown encoder key, a wrong shape or a missing encoder key raises."""
+    out, missing = _encoder_entries(sd, cfg)
+    if missing:
+        raise KeyError(f"missing encoder keys in the VAE state_dict: {_missing_text(missing)}")
+    return out
+
+
+@dataclass
+class AutoencoderKLOutput:
+    latent_dist: "DiagonalGaussianDistribution"
+
+
+class DiagonalGaussianDistribution:
+    """diffusers' posterior over the moments `parameters` [n, 8, h, w] fp16 (mean in channels 0..3, logvar in 4..7).
+    `sample` and `mode` run the vae_posterior kernel; mean / logvar / std / var are views and small tensors for callers."""
+
+    def __init__(self, parameters: torch.Tensor):
+        self.parameters = parameters
+
+    @property
+    def mean(self) -> torch.Tensor:
+        return self.parameters[:, :4]
+
+    @property
+    def logvar(self) -> torch.Tensor:
+        return self.parameters[:, 4:].clamp(-30.0, 20.0)
+
+    @property
+    def std(self) -> torch.Tensor:
+        return torch.exp(0.5 * self.logvar)
+
+    @property
+    def var(self) -> torch.Tensor:
+        return torch.exp(self.logvar)
+
+    def noise(self, generator=None) -> torch.Tensor:
+        """The standard normal draw of diffusers 0.19.3 `randn_tensor(mean.shape, generator, device, dtype=fp16)`: on the
+        generator's device when that is the CPU (then moved), one draw per frame for a list of generators."""
+        n = self.parameters.shape[0]
+        shape = (n, 4) + tuple(self.parameters.shape[2:])
+        dev = self.parameters.device
+
+        def draw(g, shp):
+            rdev = "cpu" if g is not None and g.device.type == "cpu" else dev
+            if g is not None and g.device.type != "cpu" and g.device.type != dev.type:
+                raise ValueError(f"cannot draw a {dev} tensor from a generator on {g.device}")
+            return torch.randn(shp, generator=g, device=rdev, dtype=torch.float16).to(dev)
+
+        if isinstance(generator, (list, tuple)):
+            if len(generator) != n:
+                raise ValueError(f"{len(generator)} generators for {n} frames")
+            return torch.cat([draw(g, (1,) + shape[1:]) for g in generator]).contiguous()
+        return draw(generator, shape).contiguous()
+
+    def sample(self, generator=None, scale: float = 1.0, video: bool = False) -> torch.Tensor:
+        """scale (mean + std noise) with the noise of `noise(generator)`, fp16 [n, 4, h, w] (video=True: [1, 4, n, h, w])."""
+        return ops.vae_posterior(self.parameters, self.noise(generator), scale, video)
+
+    def mode(self, scale: float = 1.0, video: bool = False) -> torch.Tensor:
+        return ops.vae_posterior(self.parameters, None, scale, video)
+
+
 def padded_keys(nk: int) -> int:
     """Row stride of S / P: O = P V runs with K = this, which the GEMM needs to be a multiple of 8."""
     return -(-nk // 8) * 8
@@ -80,8 +178,8 @@ def attend(q, k, v, s, vt, out):
 
 
 class AutoencoderKL:
-    """Decoder side of diffusers' AutoencoderKL on CUDA.  init="seeded" draws test weights (weights.seeded_state_dict),
-    "empty" waits for load_state_dict."""
+    """diffusers' AutoencoderKL (decode and encode) on CUDA.  init="seeded" draws test weights for both halves
+    (weights.seeded_state_dict), "empty" waits for load_state_dict."""
 
     def __init__(self, init: str = "seeded", device="cuda", **config):
         self.config = VAEConfig(**config)
@@ -90,8 +188,10 @@ class AutoencoderKL:
             raise ValueError("the native decoder takes 4 latent channels and makes 3 image channels")
         self.device = torch.device(device)
         self._w = None
+        self._we = None                     # encoder weights (None: the last state_dict had no complete encoder half)
+        self._enc_missing = list(vae_encoder_param_shapes(cfg))
         if init == "seeded":
-            self.load_state_dict(seeded_state_dict(vae_param_shapes(cfg), seed=7))
+            self.load_state_dict(seeded_state_dict({**vae_param_shapes(cfg), **vae_encoder_param_shapes(cfg)}, seed=7))
         elif init != "empty":
             raise ValueError(f"init must be 'seeded' or 'empty', got {init!r}")
 
@@ -128,51 +228,88 @@ class AutoencoderKL:
 
     # ------------------------------------------------------------------------------------------------ weights
     def load_state_dict(self, sd: Dict[str, torch.Tensor]):
-        """Converts (convert_state_dict) and packs every weight once: conv3x3 panels, sub-pixel panels of the up-samplers,
-        the attention's q / k / v as one [3C, C] weight, conv_out padded to 8 output channels."""
+        """Converts (convert_state_dict) and packs every decoder weight once: conv3x3 panels, sub-pixel panels of the
+        up-samplers, the attention's q / k / v as one [3C, C] weight, conv_out padded to 8 output channels.  The encoder
+        half (convert_encoder_state_dict) is packed too when sd holds all of it; otherwise `encode` raises, naming the
+        missing keys."""
         if self.device.type != "cuda":
             raise RuntimeError("AutoencoderKL (videoswap_b200) runs on CUDA only")
+        enc, self._enc_missing = _encoder_entries(sd, self.config)
         sd = convert_state_dict(sd, self.config)
+        self._w = self._pack_decoder(sd)
+        self._we = self._pack_encoder(enc) if not self._enc_missing else None
+        return self
+
+    def _loaders(self, sd):
+        """(fp16, fp32) loaders of sd's tensors onto the device."""
         dev = self.device
-        h16 = lambda k: sd[k].detach().to(dev, torch.float16).contiguous()
-        f32 = lambda k: sd[k].detach().to(dev, torch.float32).contiguous()
+        return (lambda k: sd[k].detach().to(dev, torch.float16).contiguous(),
+                lambda k: sd[k].detach().to(dev, torch.float32).contiguous())
 
-        def norm(p):
-            return f32(p + ".weight"), f32(p + ".bias")
+    def _pack_resnet(self, sd, p):
+        h16, f32 = self._loaders(sd)
 
-        def resnet(p):
-            r = {"norm1": norm(p + ".norm1"), "norm2": norm(p + ".norm2"),
-                 "conv1": (ops.pack_conv3x3(h16(p + ".conv1.weight")), f32(p + ".conv1.bias")),
-                 "conv2": (ops.pack_conv3x3(h16(p + ".conv2.weight")), f32(p + ".conv2.bias"))}
-            if p + ".conv_shortcut.weight" in sd:
-                w = h16(p + ".conv_shortcut.weight")
-                r["shortcut"] = (w.reshape(w.shape[0], w.shape[1]).contiguous(), f32(p + ".conv_shortcut.bias"))
-            return r
+        def norm(q):
+            return f32(q + ".weight"), f32(q + ".bias")
+        r = {"norm1": norm(p + ".norm1"), "norm2": norm(p + ".norm2"),
+             "conv1": (ops.pack_conv3x3(h16(p + ".conv1.weight")), f32(p + ".conv1.bias")),
+             "conv2": (ops.pack_conv3x3(h16(p + ".conv2.weight")), f32(p + ".conv2.bias"))}
+        if p + ".conv_shortcut.weight" in sd:
+            w = h16(p + ".conv_shortcut.weight")
+            r["shortcut"] = (w.reshape(w.shape[0], w.shape[1]).contiguous(), f32(p + ".conv_shortcut.bias"))
+        return r
 
-        a = "decoder.mid_block.attentions.0"
+    def _pack_attention(self, sd, a):
+        h16, f32 = self._loaders(sd)
+        return {"norm": (f32(a + ".group_norm.weight"), f32(a + ".group_norm.bias")),
+                "qkv": (torch.cat([h16(f"{a}.{n}.weight") for n in ("to_q", "to_k", "to_v")]).contiguous(),
+                        torch.cat([f32(f"{a}.{n}.bias") for n in ("to_q", "to_k", "to_v")]).contiguous()),
+                "out": (h16(a + ".to_out.0.weight"), f32(a + ".to_out.0.bias"))}
+
+    def _pack_encoder(self, sd):
+        """conv_in's [128, 3, 3, 3] weight zero-padded to 4 input channels (the tensor-core conv_in), conv3x3 panels of the
+        resnets, down-samplers and conv_out (8 output channels, no padding needed), quant_conv as fp32 weight + bias."""
+        h16, f32 = self._loaders(sd)
+        cfg = self.config
+        wi = h16("encoder.conv_in.weight")
+        wi4 = torch.zeros((wi.shape[0], 4, 3, 3), dtype=torch.float16, device=self.device)
+        wi4[:, :3] = wi
+        n = len(cfg.block_out_channels)
+        return {
+            "conv_in": (wi4, f32("encoder.conv_in.bias")),
+            "down": [{"resnets": [self._pack_resnet(sd, f"encoder.down_blocks.{i}.resnets.{j}") for j in range(cfg.layers_per_block)],
+                      "downsampler": (ops.pack_conv3x3(h16(f"encoder.down_blocks.{i}.downsamplers.0.conv.weight")),
+                                      f32(f"encoder.down_blocks.{i}.downsamplers.0.conv.bias")) if i < n - 1 else None}
+                     for i in range(n)],
+            "mid": [self._pack_resnet(sd, f"encoder.mid_block.resnets.{j}") for j in (0, 1)],
+            "attn": self._pack_attention(sd, "encoder.mid_block.attentions.0"),
+            "norm_out": (f32("encoder.conv_norm_out.weight"), f32("encoder.conv_norm_out.bias")),
+            "conv_out": (ops.pack_conv3x3(h16("encoder.conv_out.weight")), f32("encoder.conv_out.bias")),
+            "moments": torch.cat([f32("quant_conv.weight").flatten(), f32("quant_conv.bias")]).contiguous(),
+        }
+
+    def _pack_decoder(self, sd):
+        dev = self.device
+        h16, f32 = self._loaders(sd)
         cfg = self.config
         n_up = len(cfg.block_out_channels)
         w = {
             "latent_in": torch.cat([f32("post_quant_conv.weight").flatten(), f32("post_quant_conv.bias")]).contiguous(),
             "conv_in": (h16("decoder.conv_in.weight"), f32("decoder.conv_in.bias")),
-            "mid": [resnet(f"decoder.mid_block.resnets.{j}") for j in (0, 1)],
-            "attn": {"norm": norm(a + ".group_norm"),
-                     "qkv": (torch.cat([h16(f"{a}.{n}.weight") for n in ("to_q", "to_k", "to_v")]).contiguous(),
-                             torch.cat([f32(f"{a}.{n}.bias") for n in ("to_q", "to_k", "to_v")]).contiguous()),
-                     "out": (h16(a + ".to_out.0.weight"), f32(a + ".to_out.0.bias"))},
-            "up": [{"resnets": [resnet(f"decoder.up_blocks.{i}.resnets.{j}") for j in range(cfg.layers_per_block + 1)],
+            "mid": [self._pack_resnet(sd, f"decoder.mid_block.resnets.{j}") for j in (0, 1)],
+            "attn": self._pack_attention(sd, "decoder.mid_block.attentions.0"),
+            "up": [{"resnets": [self._pack_resnet(sd, f"decoder.up_blocks.{i}.resnets.{j}") for j in range(cfg.layers_per_block + 1)],
                     "upsampler": (ops.pack_conv_subpixel(h16(f"decoder.up_blocks.{i}.upsamplers.0.conv.weight")),
                                   f32(f"decoder.up_blocks.{i}.upsamplers.0.conv.bias")) if i < n_up - 1 else None}
                    for i in range(n_up)],
-            "norm_out": norm("decoder.conv_norm_out"),
+            "norm_out": (f32("decoder.conv_norm_out.weight"), f32("decoder.conv_norm_out.bias")),
         }
         wo = torch.zeros((CONV_OUT_PAD,) + tuple(sd["decoder.conv_out.weight"].shape[1:]), dtype=torch.float16, device=dev)
         wo[:cfg.out_channels] = h16("decoder.conv_out.weight")
         bo = torch.zeros(CONV_OUT_PAD, dtype=torch.float32, device=dev)
         bo[:cfg.out_channels] = f32("decoder.conv_out.bias")
         w["conv_out"] = (ops.pack_conv3x3(wo), bo)
-        self._w = w
-        return self
+        return w
 
     # ------------------------------------------------------------------------------------------------ executor
     def _groups(self):
@@ -265,3 +402,58 @@ class AutoencoderKL:
             return img
         from PIL import Image
         return [Image.fromarray(a) for a in img]
+
+    # ------------------------------------------------------------------------------------------------ encoder
+    def _encode_run(self, x, taps=None):
+        """vae_image_in -> Encoder -> quant_conv: x uint8 frames [n, H, W, 3] or float images [n, 3, H, W] in [-1, 1]
+        (CUDA) -> the moments fp16 [n, 8, H / 8, W / 8].  taps: dict that receives each block's NHWC output (debugging)."""
+        if self._we is None:
+            raise RuntimeError("AutoencoderKL has no encoder weights: the last state_dict lacked "
+                               + _missing_text(self._enc_missing))
+        if not x.is_cuda:
+            raise RuntimeError("AutoencoderKL (videoswap_b200) runs on CUDA only")
+        if x.dim() != 4:
+            raise ValueError(f"expected 4-D images, got {tuple(x.shape)}")
+        H, W = (x.shape[1], x.shape[2]) if x.dtype == torch.uint8 else (x.shape[2], x.shape[3])
+        if H % 8 or W % 8:
+            raise ValueError(f"the encoder takes images whose height and width are multiples of 8, got {tuple(x.shape)}")
+        w = self._we
+
+        def tap(name, t):
+            if taps is not None:
+                taps[name] = t
+
+        x = ops.vae_image_in(x.contiguous())
+        x = ops.conv_in(x, *w["conv_in"])
+        tap("conv_in", x)
+        for i, blk in enumerate(w["down"]):
+            for r in blk["resnets"]:
+                x = self._resnet(x, r)
+            if blk["downsampler"] is not None:
+                x = ops.downsample_conv3x3(x, *blk["downsampler"])
+            tap(f"down_blocks.{i}", x)
+        x = self._resnet(x, w["mid"][0])
+        x = self._attention(x, w["attn"])
+        tap("mid_block.attentions.0", x)
+        x = self._resnet(x, w["mid"][1])
+        tap("mid_block", x)
+        x = ops.groupnorm(x, *w["norm_out"], self._groups(), EPS, silu=True)
+        x = ops.conv3x3(x, *w["conv_out"])
+        tap("conv_out", x)
+        return ops.vae_moments(x, w["moments"])
+
+    @torch.no_grad()
+    def encode(self, x: torch.Tensor, return_dict: bool = True):
+        """AutoencoderKL.encode: CUDA images [n, 3, H, W] (fp16 / fp32, in [-1, 1]; H, W multiples of 8) ->
+        AutoencoderKLOutput(latent_dist=DiagonalGaussianDistribution) over the moments [n, 8, H / 8, W / 8]."""
+        if x.dim() != 4 or x.shape[1] != self.config.in_channels or x.dtype not in (torch.float16, torch.float32):
+            raise ValueError(f"expected fp16 / fp32 images [n, {self.config.in_channels}, H, W], got {tuple(x.shape)} {x.dtype}")
+        dist = DiagonalGaussianDistribution(self._encode_run(x))
+        return AutoencoderKLOutput(latent_dist=dist) if return_dict else (dist,)
+
+    @torch.no_grad()
+    def encode_frames(self, frames: torch.Tensor) -> DiagonalGaussianDistribution:
+        """The posterior of uint8 RGB frames [n, H, W, 3] (CUDA), normalised as VaeImageProcessor.preprocess does."""
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+            raise ValueError(f"expected uint8 frames [n, H, W, 3], got {tuple(frames.shape)} {frames.dtype}")
+        return DiagonalGaussianDistribution(self._encode_run(frames))
