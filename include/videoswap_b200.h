@@ -159,7 +159,8 @@ int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0, const voi
  *   (OH = 2H or 2H - 1, OW = 2W or 2W - 1; 0 = 2H / 2W).  Bw [N, taps (K1 + K2)], where taps = 4 except for parity 0 along
  *   an odd output axis, which has 3 taps along it (6 or 9 in all; see vs_upsample_conv3x3_sized for the panels).
  *   Epilogue: + bias[n] + rowvec[((pix / pix_per_batch) % rv_mod if rv_mod > 0), n] (row stride ldrv, 0 = N) + residual[pix, n]
- *   (row stride ldr; may alias `out`); mode 1 = GEGLU on packed weights (N / 2 output columns).  Folded LayerNorm of A:
+ *   (row stride ldr; may alias `out`); mode 1 = GEGLU on packed weights (N / 2 output columns); mode 2 = quick-GELU,
+ *   fp16(v sigmoid(1.702 v)) with v = acc + bias in fp32 (CLIP's MLP fc1: taps 1, bias only, N % 32 == 0, BLOCK_N 128 / 256).  Folded LayerNorm of A:
  *   ln_u [N] with ln_stats [M, 2] (rstd, -mean rstd) or ln_parts [ln_nparts][M][2] (sum, sum of squares).
  *   ln_sums_out [n_tiles][M][2]: (sum, sum of squares) of the stored fp16 outputs per row and column tile of width BN.
  *   force_bn 0 = automatic column-tile width, else 64 / 128 / 160 / 256.
@@ -289,8 +290,22 @@ int vs_vae_moments(void* stream, const void* d_x, int nimg, int h, int w, const 
 int vs_vae_posterior(void* stream, const void* d_params, const void* d_noise, int nimg, int h, int w, float scale, int layout,
                      void* d_out);
 
+/* ---- CLIP text encoder (transformers CLIPTextModel, SD-1.5's text_encoder; the reference's prompt encoding,
+ * pipeline_videoswap.py:273-423 and utils/edlora_util.py:116-196).  The encoder is a sequence of vs_layernorm, vs_gemm_ex
+ * (fused QKV with bias; out_proj / fc2 with bias and the in-place residual; fc1 with mode 2) and these two. */
+/* CLIPTextEmbeddings: d_out fp16 [n L, C] = fp16(fp32(d_tok[ids[s, t]]) + fp32(d_pos[t])), one rounding as torch's fp16 add.
+ * d_ids_i32 int32 [n, L] on the device, every id in [0, vocab) (the caller checks; an id outside writes NaN); d_tok fp16
+ * [vocab, C], d_pos fp16 [>= L, C]; C % 8 == 0, all three 16-byte aligned. */
+int vs_clip_embed(void* stream, const int* d_ids_i32, int n, int L, const void* d_tok, int vocab, const void* d_pos, int C,
+                  void* d_out);
+/* Causal self-attention (CLIPAttention with the causal mask, no padding mask) of nseq sequences of 1 <= L <= 77 tokens,
+ * every head of d = 64 in one launch: q / k / v of head h at columns h d, C + h d and 2 C + h d (C = heads d) of the fused
+ * QKV GEMM output d_qkv [nseq L, ldqkv] (ldqkv >= 3 C); softmax(q k^T / sqrt(d)) v of head h goes to columns h d .. h d + d - 1
+ * of d_o [nseq L, ldo].  The 1 / sqrt(d) scale is applied in fp32 inside the kernel. */
+int vs_causal_attention(void* stream, const void* d_qkv, int ldqkv, void* d_o, int ldo, int nseq, int L, int heads, int d);
+
 /* ---- measurement hooks (bench.py): per-launch CUDA-event timing on the launching stream, by kernel category
- * 0 gemm, 1 conv3x3, 2 spatial/cross attention (and the VAE's row softmax), 3 temporal attention, 4 groupnorm, 5 layernorm,
+ * 0 gemm, 1 conv3x3, 2 spatial/cross attention (and the VAE's row softmax, the CLIP causal attention), 3 temporal attention, 4 groupnorm, 5 layernorm,
  * 6 other.
  * `work` = algorithmic FLOPs (categories 0-2) or algorithmic bytes (3-5) summed over the recorded launches. */
 int vs_profile_enable(int on);

@@ -122,6 +122,8 @@ _SIGNATURES = {
     "vs_vae_image_in": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "vs_vae_moments": (_I, [_P, _P, _I, _I, _I, _P, _P]),
     "vs_vae_posterior": (_I, [_P, _P, _P, _I, _I, _I, _F, _I, _P]),
+    "vs_clip_embed": (_I, [_P, _P, _I, _I, _P, _I, _P, _I, _P]),
+    "vs_causal_attention": (_I, [_P, _P, _I, _P, _I, _I, _I, _I, _I]),
 }
 
 _lib = None

@@ -244,6 +244,14 @@ extern "C" int vs_vae_posterior(void* stream, const void* d_params, const void* 
   return vae_posterior((cudaStream_t)stream, (const __half*)d_params, (const __half*)d_noise, nimg, h, w, scale, layout,
                        (__half*)d_out);
 }
+extern "C" int vs_clip_embed(void* stream, const int* d_ids_i32, int n, int L, const void* d_tok, int vocab, const void* d_pos, int C,
+                             void* d_out) {
+  return clip_embed((cudaStream_t)stream, d_ids_i32, n, L, (const __half*)d_tok, vocab, (const __half*)d_pos, C, (__half*)d_out);
+}
+extern "C" int vs_causal_attention(void* stream, const void* d_qkv, int ldqkv, void* d_o, int ldo, int nseq, int L, int heads,
+                                   int d) {
+  return causal_attention((cudaStream_t)stream, (const __half*)d_qkv, ldqkv, (__half*)d_o, ldo, nseq, L, heads, d);
+}
 
 extern "C" int vs_profile_enable(int on) { prof_enable(on != 0); return 0; }
 extern "C" int vs_profile_reset(void) { prof_reset(); return 0; }

@@ -312,6 +312,15 @@ __device__ __forceinline__ float gelu_sig(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(xc * q));
   return __fdividef(xn, 1.f + e);
 }
+// CLIP's quick_gelu, v sigmoid(1.702 v) = v / (1 + 2^t) with t = -1.702 log2(e) v clamped at 64: for v < -26 the true
+// value is below 2e-18 and v / (1 + 2^64) is below 4e-15, both 0 in fp16; without the clamp 2^t overflows for v < -52.
+// Relative error <= 2^-21 + 2^-23 |t| <= 2^-16.9 (ex2.approx, the fp32 rounding of t, the approximate division).
+__device__ __forceinline__ float quick_gelu_f(float v) {
+  const float t = fminf(-2.4554669595930157f * v, 64.f);
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(t));
+  return __fdividef(v, 1.f + e);
+}
 #endif  // __CUDACC__
 
 }  // namespace vs

@@ -7,14 +7,15 @@
 
 namespace vs {
 
-enum EpiMode { EPI_LINEAR = 0, EPI_GEGLU = 1 };
+enum EpiMode { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_QUICK_GELU = 2 };
 
 // out[pix, n] = epilogue( sum_k A[pix(+tap shift), k] * Bw[n, k] )
 //   * plain GEMM (taps == 1): A is [M, K1] (lda1) optionally followed along K by A2 [M, K2] (channel concat).
 //   * 3x3 conv (taps == 9): A is NHWC [nimg, H, W, C1] (+ A2 [.., C2]); Bw is [N, 9*(C1+C2)], tap-major;
 //     zero padding comes from TMA out-of-bounds fill.
 //   epilogue: + bias[n] + rowvec[pix / pix_per_batch, n] + residual[pix, n]; EPI_GEGLU: value*gelu(gate) on
-//   column-interleaved weights (see pack_geglu) -> N/2 output columns.
+//   column-interleaved weights (see pack_geglu) -> N/2 output columns; EPI_QUICK_GELU: fp16((acc + bias) sigmoid(1.702
+//   (acc + bias))) (CLIP's quick_gelu; plain GEMM with a bias only, BLOCK_N 128 / 256).
 struct GemmArgs {
   const __half* A = nullptr;  int K1 = 0;  int lda1 = 0;
   const __half* A2 = nullptr; int K2 = 0;  int lda2 = 0;
@@ -101,6 +102,14 @@ int temporal_attention(cudaStream_t st, const __half* qkv, __half* o, int B, int
 int softmax_rows(cudaStream_t st, __half* s, int rows, int n, int ld, float scale);
 // dst [cols, rows_pad] = src [rows, cols]^T with zero columns rows .. rows_pad - 1.
 int transpose_pad(cudaStream_t st, const __half* src, int rows, int cols, int rows_pad, __half* dst);
+
+// ---- CLIP text encoder (text.cu) ---------------------------------------------------------------------------------
+// out [n L, C] = fp16(tok[ids[s, t]] + pos[t]) (fp32 add, one rounding); ids int32 [n, L], every id in [0, vocab).
+int clip_embed(cudaStream_t st, const int* ids, int n, int L, const __half* tok, int vocab, const __half* pos, int C,
+               __half* out);
+// Causal self-attention of nseq sequences of L <= 77 tokens: q / k / v of head h at columns h d, C + h d, 2 C + h d of
+// qkv [nseq L, ldqkv] (C = heads d, d = 64) -> o [nseq L, ldo] at column h d.
+int causal_attention(cudaStream_t st, const __half* qkv, int ldqkv, __half* o, int ldo, int nseq, int L, int heads, int d);
 
 // ---- pointwise / small -----------------------------------------------------------------------------------------
 int small_linear(cudaStream_t st, const float* x, int rows, int K, const __half* W, const float* bias, int N,

@@ -6,11 +6,12 @@
   adapter.pth        SparsePointAdapter state dict (test.py:69)                       -> `load_adapter`
   motion module ckpt AnimateDiff `mm_sd_v15*.ckpt`, keys `...pos_encoder.pe` -> `...processor.pos_encoder.pe` (test.py:62-64)
   ED-LoRA .pth       {params: {new_concept_embedding, unet, text_encoder}} (utils/convert_edlora_to_diffusers.py:84-103):
-                     W <- W + alpha * up @ down for every UNet weight that has a `lora_down` / `lora_up` pair
+                     new concept tokens and their embedding rows (`load_new_concept`), then
+                     W <- W + alpha * up @ down for every UNet / text-encoder weight that has a `lora_down` / `lora_up` pair
 
 Host-side, once per edit -- torch is the plumbing here (file I/O, a rank-4 matmul per weight); no kernel of the library is
-involved and none of this runs inside the timed step.  The text side (tokenizer, CLIP text encoder, its LoRA) and the VAE
-stay with the reference.  Nothing here imports `oracle/`.
+involved and none of this runs inside the timed step.  The text side works on the native `CLIPTextModel` (text.py) and
+the caller's tokenizer (transformers' CLIPTokenizer).  Nothing here imports `oracle/`.
 """
 from __future__ import annotations
 
@@ -100,15 +101,25 @@ def load_adapter(adapter, ckpt: PathOrDict, dtype: Optional[torch.dtype] = None)
 # ------------------------------------------------------------------------------------------------------- ED-LoRA
 _UNET_LORA_SITES = ("to_q.weight", "to_k.weight", "to_v.weight", "to_out.0.weight", "ff.net.0.proj.weight", "ff.net.2.weight",
                     "proj_out.weight", "proj_in.weight")
+_TEXT_LORA_SITES = ("q_proj.weight", "k_proj.weight", "v_proj.weight", "out_proj.weight", "fc1.weight", "fc2.weight")
+
+
+def _replace_sites(weight_name: str, sites) -> str:
+    k = weight_name
+    for site in sites:
+        k = k.replace(site, site[:-len("weight")] + "lora_down.weight")
+    return k
 
 
 def lora_down_name(weight_name: str) -> str:
     """Name of the `lora_down` tensor that would modify UNet weight `weight_name` (convert_edlora_to_diffusers.py:45-53): the
     reference applies the eight `.replace` calls IN ORDER to the whole key, so this does too."""
-    k = weight_name
-    for site in _UNET_LORA_SITES:
-        k = k.replace(site, site[:-len("weight")] + "lora_down.weight")
-    return k
+    return _replace_sites(weight_name, _UNET_LORA_SITES)
+
+
+def text_lora_down_name(weight_name: str) -> str:
+    """The same for a text-encoder weight: the six `.replace` calls of convert_edlora_to_diffusers.py:38-44, in order."""
+    return _replace_sites(weight_name, _TEXT_LORA_SITES)
 
 
 def load_edlora(ckpt: PathOrDict) -> Dict:
@@ -154,18 +165,23 @@ def merge_edlora_into_unet(unet, lora_unet: Mapping[str, torch.Tensor], alpha: f
     saved, and the returned backup restores them bit-exactly (`restore_unet`), which is what `validation()` does with its
     deep-copied state dict after every edit (pipeline_videoswap.py:303, 418).  LoRA tensors that match no weight are ignored
     like the reference ignores them (it only prints the number of merged pairs); `strict=True` raises instead."""
-    params = dict(unet.named_parameters())
+    return _merge_lora(unet, lora_unet, alpha, strict, lora_down_name, "UNet")
+
+
+def _merge_lora(model, lora: Mapping[str, torch.Tensor], alpha: float, strict: bool, down_name,
+                what: str) -> "OrderedDict[str, torch.Tensor]":
+    params = dict(model.named_parameters())
     backup: "OrderedDict[str, torch.Tensor]" = OrderedDict()
     used = set()
     for name, w in params.items():
-        dn = lora_down_name(name)
+        dn = down_name(name)
         up = dn.replace("lora_down", "lora_up")
-        if dn == name or up not in lora_unet:
+        if dn == name or up not in lora:
             continue
-        if dn not in lora_unet:
+        if dn not in lora:
             raise KeyError(f"ED-LoRA has '{up}' but not '{dn}'")
-        down_t = lora_unet[dn].to(device=w.device, dtype=torch.float32)
-        up_t = lora_unet[up].to(device=w.device, dtype=torch.float32)
+        down_t = lora[dn].to(device=w.device, dtype=torch.float32)
+        up_t = lora[up].to(device=w.device, dtype=torch.float32)
         if w.dim() == 4:
             delta = (up_t.squeeze() @ down_t.squeeze()).unsqueeze(-1).unsqueeze(-1)
         else:
@@ -175,10 +191,10 @@ def merge_edlora_into_unet(unet, lora_unet: Mapping[str, torch.Tensor], alpha: f
         backup[name] = w.detach().clone()
         w.copy_((w.to(torch.float32) + float(alpha) * delta).to(w.dtype))
         used.update((dn, up))
-    stray = [k for k in lora_unet if k not in used and ("lora_down" in k or "lora_up" in k)]
+    stray = [k for k in lora if k not in used and ("lora_down" in k or "lora_up" in k)]
     if stray and strict:
-        raise KeyError(f"{len(stray)} ED-LoRA tensors match no UNet weight, e.g. {stray[:3]}")
-    _mark_dirty(unet)
+        raise KeyError(f"{len(stray)} ED-LoRA tensors match no {what} weight, e.g. {stray[:3]}")
+    _mark_dirty(model)
     return backup
 
 
@@ -191,7 +207,43 @@ def restore_unet(unet, backup: Mapping[str, torch.Tensor]) -> None:
     _mark_dirty(unet)
 
 
-def _mark_dirty(unet):
-    mark = getattr(unet, "mark_weights_dirty", None)      # native UNet: re-pack into kernel layouts at the next forward
+def _mark_dirty(model):
+    mark = getattr(model, "mark_weights_dirty", None)     # native models: re-pack into kernel layouts at the next call
     if mark is not None:
         mark()
+
+
+@torch.no_grad()
+def merge_edlora_into_text_encoder(text_encoder, lora_te: Mapping[str, torch.Tensor], alpha: float,
+                                   strict: bool = False) -> "OrderedDict[str, torch.Tensor]":
+    """Step 3 of `convert_edlora` (convert_edlora_to_diffusers.py:98-103) in place on the text encoder's weights
+    (q / k / v / out_proj, fc1, fc2): the same single fp32 -> fp16 rounding and backup as merge_edlora_into_unet; the native
+    CLIPTextModel re-packs at its next call.  Returns the backup for restore_text_encoder."""
+    return _merge_lora(text_encoder, lora_te, alpha, strict, text_lora_down_name, "text-encoder")
+
+
+@torch.no_grad()
+def restore_text_encoder(text_encoder, backup: Mapping[str, torch.Tensor]) -> None:
+    """Undo merge_edlora_into_text_encoder bit-exactly (pipeline_videoswap.py:419 loads the pre-edit state dict without the
+    token embedding): only the merged weights are written, so concept rows of the token embedding stay."""
+    restore_unet(text_encoder, backup)
+
+
+@torch.no_grad()
+def load_new_concept(tokenizer, text_encoder, new_concept_embedding: Mapping[str, torch.Tensor],
+                     enable_edlora: bool = True) -> Dict[str, Dict[str, List]]:
+    """convert_edlora_to_diffusers.py:4-33: per concept, add its tokens `<name_i>` (16 with ED-LoRA, else 1) to the
+    tokenizer, grow the token embedding to len(tokenizer) and write the concept's rows.  Returns the reference's
+    new_concept_cfg {concept: {'concept_token_ids': [...], 'concept_token_names': [...]}}."""
+    cfg: Dict[str, Dict[str, List]] = {}
+    for concept, emb in new_concept_embedding.items():
+        names = new_concept_token_names({concept: emb}, enable_edlora)[concept]
+        added = tokenizer.add_tokens(names)
+        if added != 0 and added != len(names):
+            raise ValueError(f"some token of {concept!r} is already in the tokenizer")
+        ids = [tokenizer.convert_tokens_to_ids(n) for n in names]
+        text_encoder.resize_token_embeddings(len(tokenizer))
+        table = text_encoder.get_input_embeddings().weight.data
+        table[ids] = emb.clone().to(table.device, dtype=table.dtype)
+        cfg[concept] = {"concept_token_ids": ids, "concept_token_names": names}
+    return cfg

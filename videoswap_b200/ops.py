@@ -10,7 +10,7 @@ import torch
 from . import _lib
 
 GEGLU_GRANULE = 128
-EPI_LINEAR, EPI_GEGLU = 0, 1
+EPI_LINEAR, EPI_GEGLU, EPI_QUICK_GELU = 0, 1, 2
 
 
 def set_option(name: str, value: int):
@@ -76,7 +76,8 @@ def _gemm_ex(**fields):
 
 def gemm(A, W, bias=None, residual=None, A2=None, rowvec=None, pix_per_batch=1, mode=EPI_LINEAR, force_bn=0, out=None,
          ln_sums=None):
-    """out[M, N] = [A | A2] @ W^T (+bias +rowvec[row // pix_per_batch] +residual); GEGLU mode expects packed W/bias.
+    """out[M, N] = [A | A2] @ W^T (+bias +rowvec[row // pix_per_batch] +residual); GEGLU mode expects packed W/bias;
+    EPI_QUICK_GELU mode gives quick_gelu(A @ W^T + bias) (bias only).
     out: the caller's [M, N] ([M, N/2] for GEGLU) tensor; it may be `residual` itself (in-place residual add, as the UNet's
     attention output projections run).  rowvec may be a column slice of a wider table.  ln_sums: [slices, M, 2] fp32
     (slices >= max_column_tiles(N, force_bn)) that receives, per column tile, each row's (sum, sum of squares) of the
@@ -432,6 +433,33 @@ def vae_posterior(params, noise=None, scale=1.0, video=False):
     assert c8 == 8 and (noise is None or tuple(noise.shape) == (n, 4, h, w))
     out = torch.empty((1, 4, n, h, w) if video else (n, 4, h, w), dtype=torch.float16, device=params.device)
     _lib.call("vs_vae_posterior", _stream(), _p(params), _p(noise), n, h, w, float(scale), int(video), _p(out))
+    return out
+
+
+def clip_embed(ids, tok, pos):
+    """CLIP token + position embedding: ids int32 [n, L] (CUDA, every id in [0, tok.shape[0]) -- the caller checks), tok
+    fp16 [vocab, C], pos fp16 [>= L, C] -> fp16 [n L, C] = fp16(fp32(tok[ids]) + fp32(pos[t]))."""
+    _chk16(tok, pos)
+    assert ids.is_cuda and ids.dtype == torch.int32 and ids.is_contiguous() and ids.dim() == 2, "expected int32 [n, L] CUDA ids"
+    n, L = ids.shape
+    vocab, Cc = tok.shape
+    assert pos.shape[1] == Cc and pos.shape[0] >= L
+    out = torch.empty((n * L, Cc), dtype=torch.float16, device=tok.device)
+    _lib.call("vs_clip_embed", _stream(), _p(ids), n, L, _p(tok), vocab, _p(pos), Cc, _p(out))
+    return out
+
+
+def causal_attention(qkv, nseq, L, heads, out=None):
+    """Causal self-attention of nseq sequences of L <= 77 tokens from the fused QKV output qkv [nseq L, >= 3 C] (q, k, v
+    in column blocks of C = heads * 64; may be a column slice with unit stride) -> [nseq L, C] (`out`: the caller's tensor,
+    which may be a row-strided view)."""
+    assert qkv.is_cuda and qkv.dtype == torch.float16 and qkv.dim() == 2 and qkv.stride(1) == 1 and qkv.shape[0] == nseq * L
+    Cc = qkv.shape[1] // 3
+    if out is None:
+        out = torch.empty((nseq * L, Cc), dtype=torch.float16, device=qkv.device)
+    assert out.is_cuda and out.dtype == torch.float16 and out.stride(1) == 1 and tuple(out.shape) == (nseq * L, Cc), \
+        "out: fp16 [nseq L, C] CUDA tensor with unit column stride"
+    _lib.call("vs_causal_attention", _stream(), _p(qkv), qkv.stride(0), _p(out), out.stride(0), nseq, L, heads, Cc // heads)
     return out
 
 

@@ -2,10 +2,10 @@
 denoising part of `VideoSwapPipeline` (videoswap/pipelines/pipeline_videoswap.py:427-619 `__call__`, :622-721 `invert`).
 
 Scope (SURVEY.md 8): the loop body -- CFG batch duplication, UNet forward, CFG combine, scheduler step, adapter
-residual window -- runs on the native kernels.  Text encoding (CLIP) and prompt/LoRA handling are callers on either side
-of this path (8f) and are NOT part of this package: the pipeline takes `prompt_embeds` and `latents` tensors and returns
-latents.  Given a `vae` (videoswap_b200.vae.AutoencoderKL) it also encodes the source frames for the DDIM inversion
-(`prepare_image_latents`, `invert(video=...)`) and decodes the result into frames.
+residual window -- runs on the native kernels.  The pipeline takes `prompt_embeds` and `latents` tensors and returns
+latents.  Given a `text_encoder` (videoswap_b200.text.CLIPTextModel) and the caller's `tokenizer` it also takes prompts
+(`encode_prompt`, plain or ED-LoRA); given a `vae` (videoswap_b200.vae.AutoencoderKL) it encodes the source frames for the
+DDIM inversion (`prepare_image_latents`, `invert(video=...)`) and decodes the result into frames.
 """
 from __future__ import annotations
 
@@ -16,6 +16,7 @@ import torch
 from torch import nn
 
 from . import ops
+from .formats import bind_concept_prompt
 from .scheduler import DDIMInverseScheduler, DDIMScheduler
 from .spec import adapter_param_shapes
 from .unet import AnimateDiffUNet3DModel, _Holder
@@ -121,14 +122,66 @@ class VideoSwapPipeline:
 
     def __init__(self, unet: AnimateDiffUNet3DModel, scheduler: Optional[DDIMScheduler] = None,
                  adapter: Optional[SparsePointAdapter] = None, inverse_scheduler: Optional[DDIMInverseScheduler] = None,
-                 vae: Optional[AutoencoderKL] = None):
+                 vae: Optional[AutoencoderKL] = None, text_encoder=None, tokenizer=None):
         """vae: encodes the source video for the inversion (invert(video=...)) and turns the final latents into frames
-        (output_type "pt" / "np" / "pil"); without it the pipeline takes and returns latents only."""
+        (output_type "pt" / "np" / "pil"); without it the pipeline takes and returns latents only.
+        text_encoder (text.CLIPTextModel) + tokenizer (transformers' CLIPTokenizer, or anything with its call interface):
+        `prompt=` instead of `prompt_embeds` (encode_prompt)."""
         self.unet = unet
         self.scheduler = scheduler or DDIMScheduler()
         self.inverse_scheduler = inverse_scheduler or DDIMInverseScheduler()
         self.adapter = adapter
         self.vae = vae
+        self.text_encoder = text_encoder
+        self.tokenizer = tokenizer
+        self.new_concept_cfg = None
+
+    def set_new_concept_cfg(self, new_concept_cfg=None):
+        """ED-LoRA concepts (formats.load_new_concept) that encode_prompt binds into 16 per-layer prompts; None: plain
+        prompts (pipeline_videoswap.py:174-176)."""
+        self.new_concept_cfg = new_concept_cfg
+
+    def _encode(self, texts: List[str]) -> torch.Tensor:
+        """One batch through the text encoder: tokenizer(padding="max_length", max_length=model_max_length, truncation)
+        -> last_hidden_state [len(texts), 77, 768]."""
+        if self.text_encoder is None or self.tokenizer is None:
+            raise ValueError("prompts need a VideoSwapPipeline(..., text_encoder=CLIPTextModel, tokenizer=CLIPTokenizer)")
+        ids = self.tokenizer(texts, padding="max_length", max_length=self.tokenizer.model_max_length, truncation=True,
+                             return_tensors="pt").input_ids
+        return self.text_encoder(ids)[0]
+
+    @torch.no_grad()
+    def encode_prompt(self, prompt, negative_prompt=None, do_classifier_free_guidance: bool = True,
+                      plain: bool = False) -> torch.Tensor:
+        """Prompt embeddings, every sequence of the call in one encoder batch, uncond first under CFG:
+          * no concept config (or plain=True): diffusers 0.19.3 `_encode_prompt` -> [2 b, 77, 768] (cat(neg, pos); the
+            negative defaults to "");
+          * with set_new_concept_cfg: `encode_edlora_prompt` (edlora_util.py:116-196) -> [2 b, 16, 77, 768]: each prompt
+            bound into 16 per-layer prompts (formats.bind_concept_prompt), each negative encoded once and repeated 16 times.
+        Without CFG the uncond half is left out."""
+        prompts = [prompt] if isinstance(prompt, str) else list(prompt)
+        b = len(prompts)
+        uncond: List[str] = []
+        if do_classifier_free_guidance:
+            if negative_prompt is None:
+                uncond = [""] * b
+            elif type(prompt) is not type(negative_prompt):
+                raise TypeError(f"negative_prompt should be the same type as prompt, got {type(negative_prompt)} != {type(prompt)}")
+            elif isinstance(negative_prompt, str):
+                uncond = [negative_prompt]
+            elif len(negative_prompt) != b:
+                raise ValueError(f"negative_prompt has batch size {len(negative_prompt)}, prompt has {b}")
+            else:
+                uncond = list(negative_prompt)
+        if plain or self.new_concept_cfg is None:
+            return self._encode(uncond + prompts)
+        emb = self._encode(bind_concept_prompt(prompts, self.new_concept_cfg) + uncond)
+        L, C = emb.shape[1:]
+        pos = emb[:16 * b].view(b, 16, L, C)
+        if not do_classifier_free_guidance:
+            return pos
+        neg = emb[16 * b:].view(b, 1, L, C).repeat(1, 16, 1, 1)
+        return torch.cat([neg, pos])
 
     @property
     def device(self):
@@ -177,14 +230,22 @@ class VideoSwapPipeline:
         return _combine(eps, latents, guidance_scale, a_t, a_p, cfg)
 
     @torch.no_grad()
-    def __call__(self, prompt_embeds: torch.Tensor, latents: torch.Tensor, negative_prompt_embeds: Optional[torch.Tensor] = None,
+    def __call__(self, prompt_embeds: Optional[torch.Tensor] = None, latents: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None,
                  conditions: Optional[Dict] = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
                  t2i_guidance_scale: float = 1.0, t2i_start: float = 0.0, t2i_end: float = 1.0, controller=None,
                  output_type: str = "latent", return_dict: bool = True, callback=None, callback_steps: int = 1,
-                 max_iters: Optional[int] = None):
+                 max_iters: Optional[int] = None, *, prompt=None, negative_prompt=None):
         """prompt_embeds: [1,77,D] / ED-LoRA [1,16,77,D] (conditional); negative_prompt_embeds same shape (uncond).
+        Or `prompt` (+ `negative_prompt`), encoded with encode_prompt (exactly one of prompt and prompt_embeds).
         latents [1,4,F,h,w] (e.g. DDIM-inverted).  Mirrors pipeline_videoswap.py:552-610: output_type "latent" returns
         the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents)."""
+        if (prompt is None) == (prompt_embeds is None):
+            raise ValueError("give exactly one of `prompt` and `prompt_embeds`")
+        if prompt is not None and negative_prompt_embeds is not None:
+            raise ValueError("`prompt` takes `negative_prompt`, not `negative_prompt_embeds`")
+        if latents is None:
+            raise ValueError("VideoSwapPipeline needs `latents` (e.g. from invert)")
         if output_type != "latent":
             if self.vae is None:
                 raise NotImplementedError("decoding needs a VideoSwapPipeline(..., vae=AutoencoderKL); use output_type='latent'")
@@ -192,7 +253,9 @@ class VideoSwapPipeline:
                 raise ValueError(f"output_type must be 'latent', 'pt', 'np' or 'pil', got {output_type!r}")
         cfg = guidance_scale > 1.0
         dev = latents.device
-        if cfg:
+        if prompt is not None:
+            embeds = self.encode_prompt(prompt, negative_prompt, cfg)           # uncond first under CFG
+        elif cfg:
             if negative_prompt_embeds is None:
                 raise ValueError("classifier-free guidance needs negative_prompt_embeds")
             embeds = torch.cat([negative_prompt_embeds, prompt_embeds], dim=0)     # uncond FIRST (edlora_util.py:190-195)
@@ -270,13 +333,20 @@ class VideoSwapPipeline:
         return dist.sample(generator, scale=self.vae.config.scaling_factor, video=True)
 
     @torch.no_grad()
-    def invert(self, prompt_embeds: torch.Tensor, latents: Optional[torch.Tensor] = None, num_inference_steps: int = 50,
-               return_dict: bool = True, controller=None, max_iters: Optional[int] = None, *, video=None, generator=None):
+    def invert(self, prompt_embeds: Optional[torch.Tensor] = None, latents: Optional[torch.Tensor] = None,
+               num_inference_steps: int = 50, return_dict: bool = True, controller=None, max_iters: Optional[int] = None, *,
+               video=None, generator=None, prompt=None):
         """DDIM inversion loop (pipeline_videoswap.py:677-703), guidance_scale = 1 (no CFG).  The UNet is evaluated at
         the inverse scheduler's timestep; which noise levels the step connects is the scheduler's `convention`.
-        Exactly one of `latents` ([1, 4, F, h, w]) and `video` (see prepare_image_latents, with `generator`) is given."""
+        Exactly one of `latents` ([1, 4, F, h, w]) and `video` (see prepare_image_latents, with `generator`) is given, and
+        exactly one of `prompt_embeds` and `prompt`; a prompt is encoded plainly even with a concept config, as the
+        reference's invert does (pipeline_videoswap.py:658)."""
+        if (prompt is None) == (prompt_embeds is None):
+            raise ValueError("give exactly one of `prompt` and `prompt_embeds`")
         if (latents is None) == (video is None):
             raise ValueError("invert takes exactly one of `latents` and `video`")
+        if prompt is not None:
+            prompt_embeds = self.encode_prompt(prompt, do_classifier_free_guidance=False, plain=True)
         if video is not None:
             latents = self.prepare_image_latents(video, generator)
         self.inverse_scheduler.set_timesteps(num_inference_steps)

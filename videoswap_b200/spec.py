@@ -286,3 +286,44 @@ def adapter_param_shapes(embedding_channels=1280, channels=(320, 640, 1280, 1280
         sh[f"model_list.{l}.mlp.2.weight"] = (ch, mid_dim)
         sh[f"model_list.{l}.mlp.2.bias"] = (ch,)
     return sh
+
+
+@dataclass
+class CLIPTextConfig:
+    """The fields of SD-1.5's text_encoder/config.json (transformers CLIPTextConfig) that shape the model."""
+    vocab_size: int = 49408
+    hidden_size: int = 768
+    intermediate_size: int = 3072
+    num_hidden_layers: int = 12
+    num_attention_heads: int = 12
+    max_position_embeddings: int = 77
+    hidden_act: str = "quick_gelu"
+    layer_norm_eps: float = 1e-5
+
+    def to_dict(self):
+        return asdict(self)
+
+
+def clip_text_param_shapes(cfg: CLIPTextConfig = CLIPTextConfig()) -> "OrderedDict[str, Tuple[int, ...]]":
+    """CLIPTextModel.state_dict() keys and shapes (transformers modeling_clip.py) without the `position_ids` buffer that
+    older checkpoints carry: 196 tensors and 123,060,480 parameters for SD-1.5."""
+    C, F = cfg.hidden_size, cfg.intermediate_size
+    sh: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    sh["text_model.embeddings.token_embedding.weight"] = (cfg.vocab_size, C)
+    sh["text_model.embeddings.position_embedding.weight"] = (cfg.max_position_embeddings, C)
+    for i in range(cfg.num_hidden_layers):
+        p = f"text_model.encoder.layers.{i}"
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            sh[f"{p}.self_attn.{n}.weight"] = (C, C)
+            sh[f"{p}.self_attn.{n}.bias"] = (C,)
+        sh[f"{p}.layer_norm1.weight"] = (C,)
+        sh[f"{p}.layer_norm1.bias"] = (C,)
+        sh[f"{p}.mlp.fc1.weight"] = (F, C)
+        sh[f"{p}.mlp.fc1.bias"] = (F,)
+        sh[f"{p}.mlp.fc2.weight"] = (C, F)
+        sh[f"{p}.mlp.fc2.bias"] = (C,)
+        sh[f"{p}.layer_norm2.weight"] = (C,)
+        sh[f"{p}.layer_norm2.bias"] = (C,)
+    sh["text_model.final_layer_norm.weight"] = (C,)
+    sh["text_model.final_layer_norm.bias"] = (C,)
+    return sh
