@@ -72,6 +72,15 @@ const char* vs_unet_param_name(const vs_unet* h, int i);
 int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
                     const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers,
                     const void* const* d_residuals, int residuals_nhwc, float residual_scale, void* d_out);
+/* The DIFT featurizer (the reference's dift_util.py MyUNet2DConditionModel): the same forward as a UNet2DConditionModel --
+ * time embedding, conv_in, down path, mid block and up blocks 0..up_ft_index, WITHOUT any motion module -- stopping after
+ * up block up_ft_index and its up-sampler (the reference's up_ft[up_ft_index]).  Pass F = 1 with every image on B, so the
+ * ResNet GroupNorm statistics are per image as in the 2-D UNet.  d_feat: NHWC fp16 [B F, h_k, w_k, C_k], C_k =
+ * block_out_channels[3 - k] at level 2 - k for k < 3 (block_out_channels[0] at level 0 for k = 3), on the level sizes of
+ * vs_unet_forward.  Fails before any launch for up_ft_index outside 0..3, a frame-sharded handle or a set attention hook. */
+int vs_unet_forward_features(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
+                             const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers, int up_ft_index,
+                             void* d_feat);
 size_t vs_unet_workspace_bytes(const vs_unet* h);
 /* The activation workspace is one arena that only grows: a forward of a smaller shape re-uses it.  A captured CUDA graph
  * holds raw pointers into it, so the owner of a graph pins the arena (pin != 0; unpin with 0 when the graph dies): while
@@ -303,6 +312,25 @@ int vs_clip_embed(void* stream, const int* d_ids_i32, int n, int L, const void* 
  * QKV GEMM output d_qkv [nseq L, ldqkv] (ldqkv >= 3 C); softmax(q k^T / sqrt(d)) v of head h goes to columns h d .. h d + d - 1
  * of d_o [nseq L, ldo].  The 1 / sqrt(d) scale is applied in fp32 inside the kernel. */
 int vs_causal_attention(void* stream, const void* d_qkv, int ldqkv, void* d_o, int ldo, int nseq, int L, int heads, int d);
+
+/* ---- DIFT semantic points (the reference's dift_util.py / extract_semantic_point.py:125-204) ----------------------------
+ * d_out fp32 [n E, 4, h, w] = sqrt_a sf (mu + exp(0.5 clamp(logvar, -30, 20)) eps1) + sqrt_1ma eps2: the posterior draw of
+ * frame r / E (moments fp16 [n, 8, h, w] of vs_vae_moments) then DDPM add_noise; d_eps1, d_eps2 fp32 [n E, 4, h, w]. */
+int vs_dift_noise(void* stream, const void* d_moments, const float* d_eps1, const float* d_eps2, int n, int E, int h, int w,
+                  float sf, float sqrt_a, float sqrt_1ma, float* d_out);
+/* d_out fp32 [n, P, C]: the ensemble mean of d_feat (NHWC fp16 [n, E, h, w, C], C % 8 == 0) up-sampled as
+ * nn.Upsample(size=(H, W), mode="bilinear") and read at the pixels d_xy int32 [n, P, 2] = (x, y), 0 <= x < W, 0 <= y < H.
+ * Source indices and interpolation order are those of torch's CPU upsample_bilinear2d in fp32; no map is materialised. */
+int vs_dift_point_sample(void* stream, const void* d_feat, int n, int E, int h, int w, int C, int H, int W, const int* d_xy,
+                         int P, float* d_out);
+/* d_out fp32 NCHW [n, C, h, w] = the mean over E of d_feat NHWC fp16 [n, E, h, w, C] (SDFeaturizer.forward's map). */
+int vs_dift_ensemble_mean(void* stream, const void* d_feat, int n, int E, int h, int w, int C, float* d_out);
+/* d_vecs fp32 [n, P, C].  With d_src (fp32 rows [*, C]), d_src_row int32 [n, P] and d_conf fp32 [n, P]: the cosine
+ * similarity (CosineSimilarity(dim=1, eps=1e-8)) of each vector against its source row.  With d_accept uint8 [n, P]: the
+ * per-point sums / means fp32 [P, C] and counts fp32 [P] over the accepted frames, accumulated in frame order (each of the
+ * three may be NULL; a point never accepted has mean 0). */
+int vs_dift_point_reduce(void* stream, const float* d_vecs, int n, int P, int C, const float* d_src, const int* d_src_row,
+                         float* d_conf, const void* d_accept, float* d_sums, float* d_counts, float* d_means);
 
 /* ---- measurement hooks (bench.py): per-launch CUDA-event timing on the launching stream, by kernel category
  * 0 gemm, 1 conv3x3, 2 spatial/cross attention (and the VAE's row softmax, the CLIP causal attention), 3 temporal attention, 4 groupnorm, 5 layernorm,

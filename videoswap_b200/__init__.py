@@ -1,8 +1,10 @@
 """videoswap_b200: H100-native (sm_90a) implementation of the denoising hot path of showlab/VideoSwap -- the
 `AnimateDiffUNet3DModel` forward + classifier-free guidance + DDIM step, the CLIP text encoder of the prompts, the VAE
-encode of the source frames and the VAE decode of the result -- behind the reference's own Python surface.
+encode of the source frames, the VAE decode of the result and the DIFT features of tracked points -- behind the
+reference's own Python surface.
 See DESIGN.md / INTEGRATION.md.  Importing this package never touches `oracle/` and there is no CPU fallback."""
 from . import formats  # noqa: F401
+from .dift import DIFT_Demo, SDFeaturizer, extract_point_embedding  # noqa: F401
 from .pipeline import (SparsePointAdapter, TuneAVideoPipeline, TuneAVideoPipelineOutput, VideoSwapPipeline)  # noqa: F401
 from .scheduler import DDIMInverseScheduler, DDIMScheduler  # noqa: F401
 from .spec import (CLIPTextConfig, UNetConfig, VAEConfig, adapter_param_shapes, clip_text_param_shapes,  # noqa: F401

@@ -124,6 +124,11 @@ _SIGNATURES = {
     "vs_vae_posterior": (_I, [_P, _P, _P, _I, _I, _I, _F, _I, _P]),
     "vs_clip_embed": (_I, [_P, _P, _I, _I, _P, _I, _P, _I, _P]),
     "vs_causal_attention": (_I, [_P, _P, _I, _P, _I, _I, _I, _I, _I]),
+    "vs_unet_forward_features": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P]),
+    "vs_dift_noise": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _F, _F, _P]),
+    "vs_dift_point_sample": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "vs_dift_ensemble_mean": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
+    "vs_dift_point_reduce": (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
 }
 
 _lib = None

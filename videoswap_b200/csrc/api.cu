@@ -253,6 +253,24 @@ extern "C" int vs_causal_attention(void* stream, const void* d_qkv, int ldqkv, v
   return causal_attention((cudaStream_t)stream, (const __half*)d_qkv, ldqkv, (__half*)d_o, ldo, nseq, L, heads, d);
 }
 
+extern "C" int vs_dift_noise(void* stream, const void* d_moments, const float* d_eps1, const float* d_eps2, int n, int E, int h,
+                             int w, float sf, float sqrt_a, float sqrt_1ma, float* d_out) {
+  return dift_noise((cudaStream_t)stream, (const __half*)d_moments, d_eps1, d_eps2, n, E, h, w, sf, sqrt_a, sqrt_1ma, d_out);
+}
+extern "C" int vs_dift_point_sample(void* stream, const void* d_feat, int n, int E, int h, int w, int C, int H, int W,
+                                    const int* d_xy, int P, float* d_out) {
+  return dift_point_sample((cudaStream_t)stream, (const __half*)d_feat, n, E, h, w, C, H, W, d_xy, P, d_out);
+}
+extern "C" int vs_dift_ensemble_mean(void* stream, const void* d_feat, int n, int E, int h, int w, int C, float* d_out) {
+  return dift_ensemble_mean((cudaStream_t)stream, (const __half*)d_feat, n, E, h, w, C, d_out);
+}
+extern "C" int vs_dift_point_reduce(void* stream, const float* d_vecs, int n, int P, int C, const float* d_src,
+                                    const int* d_src_row, float* d_conf, const void* d_accept, float* d_sums, float* d_counts,
+                                    float* d_means) {
+  return dift_point_reduce((cudaStream_t)stream, d_vecs, n, P, C, d_src, d_src_row, d_conf, (const uint8_t*)d_accept, d_sums,
+                           d_counts, d_means);
+}
+
 extern "C" int vs_profile_enable(int on) { prof_enable(on != 0); return 0; }
 extern "C" int vs_profile_reset(void) { prof_reset(); return 0; }
 extern "C" int vs_profile_collect(int category, double* ms, double* work, long long* count) {

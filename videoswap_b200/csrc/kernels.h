@@ -111,6 +111,22 @@ int clip_embed(cudaStream_t st, const int* ids, int n, int L, const __half* tok,
 // qkv [nseq L, ldqkv] (C = heads d, d = 64) -> o [nseq L, ldo] at column h d.
 int causal_attention(cudaStream_t st, const __half* qkv, int ldqkv, __half* o, int ldo, int nseq, int L, int heads, int d);
 
+// ---- DIFT semantic points (dift.cu) ----------------------------------------------------------------------------------
+// out fp32 [n E, 4, h, w] = sqrt_a sf (mu + exp(0.5 clamp(logvar, -30, 20)) eps1) + sqrt_1ma eps2, with mu / logvar of
+// frame (row / E) from the VAE moments fp16 [n, 8, h, w]; eps1, eps2 fp32 [n E, 4, h, w].
+int dift_noise(cudaStream_t st, const __half* moments, const float* eps1, const float* eps2, int n, int E, int h, int w,
+               float sf, float sqrt_a, float sqrt_1ma, float* out);
+// out fp32 [n, P, C]: ensemble mean of feat NHWC fp16 [n, E, h, w, C] up-sampled bilinearly (align_corners False) to
+// H x W, read at the pixels xy int32 [n, P, 2] = (x, y) in [0, W) x [0, H) (torch's CPU source-index arithmetic).  C % 8 == 0.
+int dift_point_sample(cudaStream_t st, const __half* feat, int n, int E, int h, int w, int C, int H, int W, const int* xy,
+                      int P, float* out);
+// out fp32 NCHW [n, C, h, w] = mean over E of feat NHWC fp16 [n, E, h, w, C]
+int dift_ensemble_mean(cudaStream_t st, const __half* feat, int n, int E, int h, int w, int C, float* out);
+// vecs fp32 [n, P, C].  With src: conf[f, p] = cosine(vecs[f, p], src[src_row[f P + p]]) (eps 1e-8).  With accept uint8
+// [n, P]: sums / means [P, C] and counts [P] over the accepted frames, in frame order (any of the three may be null).
+int dift_point_reduce(cudaStream_t st, const float* vecs, int n, int P, int C, const float* src, const int* src_row,
+                      float* conf, const uint8_t* accept, float* sums, float* counts, float* means);
+
 // ---- pointwise / small -----------------------------------------------------------------------------------------
 int small_linear(cudaStream_t st, const float* x, int rows, int K, const __half* W, const float* bias, int N,
                  bool silu_in, bool silu_out, float* out);     // out[r,n] = act(sum_k f(x[r,k]) W[n,k] + b[n]), fp32

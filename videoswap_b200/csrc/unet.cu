@@ -740,9 +740,13 @@ extern "C" int vs_unet_copy_tap(const vs_unet* h, void* stream, int i, void* d_d
   return 0;
 }
 
-extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
-                               const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers,
-                               const void* const* d_residuals, int residuals_nhwc, float residual_scale, void* d_out) {
+namespace {
+
+// The body of vs_unet_forward.  stop_up >= 0 (vs_unet_forward_features) runs the 2-D UNet: no motion module, and the walk
+// ends after up block `stop_up` (with its up-sampler), whose output is copied to d_out as NHWC fp16.
+int unet_run(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W, const float* d_timesteps,
+             const void* d_ehs, int ehs_tokens, int ehs_layers, const void* const* d_residuals, int residuals_nhwc,
+             float residual_scale, int stop_up, void* d_out) {
   VS_REQUIRE(h && d_sample && d_timesteps && d_ehs && d_out, "vs_unet_forward: null argument");
   VS_REQUIRE(B >= 1 && F >= 1 && H >= 1 && W >= 1, "vs_unet_forward: bad shape");
   VS_REQUIRE(ehs_tokens >= 1 && ehs_tokens <= 128, "vs_unet_forward: ehs_tokens out of range");
@@ -808,7 +812,7 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
       RUN(resnet(c, L.res, cur, curC, nullptr, 0, out));
       curC = L.res.cout;
       if (L.has_tr) RUN(transformer(c, L.tr, out));
-      if (L.has_mo) RUN(motion(c, L.mo, i, out));
+      if (L.has_mo && stop_up < 0) RUN(motion(c, L.mo, i, out));
       if (i < 3 && j == lpb - 1 && res_l) {
         const size_t n = (size_t)c.NI * c.H * c.W * curC;
         if (!residuals_nhwc) RUN(nchw_to_nhwc(st, (const __half*)d_residuals[i], c.NI, curC, c.H, c.W, residual_scale, h->RES));
@@ -847,7 +851,7 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
     __half* o = (cur == h->P0) ? h->P1 : h->P0;
     RUN(resnet(c, h->mid0.res, cur, curC, nullptr, 0, o));
     RUN(transformer(c, h->mid0.tr, o));
-    if (h->mid0.has_mo) RUN(motion(c, h->mid0.mo, 3, o));
+    if (h->mid0.has_mo && stop_up < 0) RUN(motion(c, h->mid0.mo, 3, o));
     __half* o2 = (o == h->P0) ? h->P1 : h->P0;
     RUN(resnet(c, h->mid1, o, curC, nullptr, 0, o2));
     RUN(tap(c, "mid_block", o2, curC));
@@ -865,7 +869,7 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
       RUN(resnet(c, L.res, cur, curC, sk.first, sk.second, o));
       curC = L.res.cout;
       if (L.has_tr) RUN(transformer(c, L.tr, o));
-      if (L.has_mo) RUN(motion(c, L.mo, 3 - i, o));
+      if (L.has_mo && stop_up < 0) RUN(motion(c, L.mo, 3 - i, o));
       RUN(tap(c, "up_blocks." + std::to_string(i) + "." + std::to_string(j), o, curC));
       cur = o;
     }
@@ -886,6 +890,10 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
       }
       cur = o;
     }
+    if (i == stop_up) {              // up_ft[i] of the DIFT featurizer: the block's output after its up-sampler
+      VS_CHECK_CUDA(cudaMemcpyAsync(d_out, cur, (size_t)c.NI * c.H * c.W * curC * 2, cudaMemcpyDeviceToDevice, st));
+      return 0;
+    }
   }
   VS_REQUIRE(c.H == H && c.W == W, "internal: the up path ended at %dx%d, not at the input's %dx%d", c.H, c.W, H, W);
   // ---- out: GroupNorm(5-D) + SiLU + conv_out
@@ -903,4 +911,24 @@ extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, i
   RUN(tap(c, "conv_out", h->OUT, cf.out_channels));
   RUN(nhwc_to_ncfhw(st, h->OUT, B, cf.out_channels, F, H, W, d_out, io_f32));
   return 0;
+}
+
+}  // namespace
+
+extern "C" int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
+                               const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers,
+                               const void* const* d_residuals, int residuals_nhwc, float residual_scale, void* d_out) {
+  return unet_run(h, stream, d_sample, io_f32, B, F, H, W, d_timesteps, d_ehs, ehs_tokens, ehs_layers, d_residuals,
+                  residuals_nhwc, residual_scale, -1, d_out);
+}
+
+extern "C" int vs_unet_forward_features(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
+                                        const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers,
+                                        int up_ft_index, void* d_feat) {
+  VS_REQUIRE(h && d_feat, "vs_unet_forward_features: null argument");
+  VS_REQUIRE(up_ft_index >= 0 && up_ft_index <= 3, "vs_unet_forward_features: up_ft_index %d is outside 0..3", up_ft_index);
+  VS_REQUIRE(h->fnshards == 1, "vs_unet_forward_features: the featurizer runs unsharded (frame sharding is set)");
+  VS_REQUIRE(h->hook == nullptr, "vs_unet_forward_features: the featurizer runs without attention controllers (a hook is set)");
+  return unet_run(h, stream, d_sample, io_f32, B, F, H, W, d_timesteps, d_ehs, ehs_tokens, ehs_layers, nullptr, 0, 1.f,
+                  up_ft_index, d_feat);
 }

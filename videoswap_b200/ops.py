@@ -535,3 +535,67 @@ def adapter_level(w0, b0, w1, b1, point_embedding, tracks, h, w, rate, point_mas
     _lib.call("vs_adapter_level", _stream(), _p(w0), _p(b0), _p(w1), _p(b1), E, mid, Cc, _p(point_embedding), _p(tracks),
               _p(point_mask), F, P, h, w, float(rate), int(coord_fp16), float(scale), _p(ws), _p(out))
     return out
+
+
+def dift_noise(moments, eps1, eps2, scaling_factor, sqrt_a, sqrt_1ma):
+    """The DIFT UNet input fp32 [n E, 4, 1, h, w] = sqrt_a sf (mean + std eps1) + sqrt_1ma eps2 from the VAE moments
+    fp16 [n, 8, h, w] of n frames and fp32 noise eps1, eps2 [n E, 4, h, w] (row r belongs to frame r // E)."""
+    _chk16(moments)
+    _chk32(eps1, eps2)
+    n, c8, h, w = moments.shape
+    assert c8 == 8 and eps1.shape == eps2.shape and eps1.dim() == 4 and tuple(eps1.shape[1:]) == (4, h, w)
+    assert eps1.shape[0] % n == 0, "noise rows must be a whole ensemble per frame"
+    E = eps1.shape[0] // n
+    out = torch.empty((n * E, 4, 1, h, w), dtype=torch.float32, device=moments.device)
+    _lib.call("vs_dift_noise", _stream(), _p(moments), _p(eps1), _p(eps2), n, E, h, w, float(scaling_factor), float(sqrt_a),
+              float(sqrt_1ma), _p(out))
+    return out
+
+
+def dift_point_sample(feat, size, xy):
+    """Ensemble mean of feat NHWC fp16 [n, E, h, w, C] up-sampled bilinearly (align_corners False) to size = (H, W),
+    read at the pixels xy int32 [n, P, 2] = (x, y) inside the image -> fp32 [n, P, C]."""
+    _chk16(feat)
+    assert xy.is_cuda and xy.dtype == torch.int32 and xy.is_contiguous() and xy.dim() == 3 and xy.shape[2] == 2
+    n, E, h, w, Cc = feat.shape
+    assert xy.shape[0] == n
+    P = xy.shape[1]
+    out = torch.empty((n, P, Cc), dtype=torch.float32, device=feat.device)
+    if P:
+        _lib.call("vs_dift_point_sample", _stream(), _p(feat), n, E, h, w, Cc, int(size[0]), int(size[1]), _p(xy), P, _p(out))
+    return out
+
+
+def dift_ensemble_mean(feat):
+    """feat NHWC fp16 [n, E, h, w, C] -> fp32 NCHW [n, C, h, w], the mean over E."""
+    _chk16(feat)
+    n, E, h, w, Cc = feat.shape
+    out = torch.empty((n, Cc, h, w), dtype=torch.float32, device=feat.device)
+    _lib.call("vs_dift_ensemble_mean", _stream(), _p(feat), n, E, h, w, Cc, _p(out))
+    return out
+
+
+def dift_point_cosine(vecs, src, src_row):
+    """CosineSimilarity(dim=1, eps=1e-8) of vecs fp32 [n, P, C] against src[src_row] (src fp32 [S, C], src_row int32
+    [n, P]) -> fp32 [n, P]."""
+    _chk32(vecs, src)
+    assert src_row.is_cuda and src_row.dtype == torch.int32 and src_row.is_contiguous()
+    n, P, Cc = vecs.shape
+    assert src.dim() == 2 and src.shape[1] == Cc and tuple(src_row.shape) == (n, P)
+    conf = torch.empty((n, P), dtype=torch.float32, device=vecs.device)
+    _lib.call("vs_dift_point_reduce", _stream(), _p(vecs), n, P, Cc, _p(src), _p(src_row), _p(conf), None, None, None, None)
+    return conf
+
+
+def dift_point_reduce(vecs, accept):
+    """Per-point (sums [P, C], counts [P], means [P, C]) fp32 of vecs fp32 [n, P, C] over the frames where accept (bool /
+    uint8 [n, P]) is set, accumulated in frame order; a point never accepted has mean 0."""
+    _chk32(vecs)
+    n, P, Cc = vecs.shape
+    acc = accept.to(device=vecs.device, dtype=torch.uint8).contiguous()
+    assert tuple(acc.shape) == (n, P)
+    sums = torch.empty((P, Cc), dtype=torch.float32, device=vecs.device)
+    means = torch.empty_like(sums)
+    counts = torch.empty((P,), dtype=torch.float32, device=vecs.device)
+    _lib.call("vs_dift_point_reduce", _stream(), _p(vecs), n, P, Cc, None, None, None, _p(acc), _p(sums), _p(counts), _p(means))
+    return sums, counts, means

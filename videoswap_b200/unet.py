@@ -576,4 +576,45 @@ class AnimateDiffUNet3DModel(nn.Module):
         return UNet3DConditionOutput(sample=out)
 
 
+    @torch.no_grad()
+    def forward_features(self, sample: torch.Tensor, timestep: Union[torch.Tensor, float, int],
+                         encoder_hidden_states: torch.Tensor, up_ft_index: int = 1) -> torch.Tensor:
+        """The DIFT featurizer's partial forward (dift_util.py MyUNet2DConditionModel): the 2-D UNet -- every motion
+        module skipped -- up to and including up block `up_ft_index` with its up-sampler.  sample [N, C, 1, H, W] (fp16 /
+        fp32; every image on the batch axis, so each one gets its own GroupNorm statistics), encoder_hidden_states
+        [N, 77, D] -> up_ft[up_ft_index] as NHWC fp16 [N, h_k, w_k, C_k]."""
+        if not sample.is_cuda:
+            raise RuntimeError("AnimateDiffUNet3DModel (videoswap_b200) runs on CUDA only: there is no CPU path")
+        if sample.dim() != 5 or sample.shape[2] != 1 or sample.shape[1] != self.cfg.in_channels:
+            raise ValueError(f"expected sample [N, {self.cfg.in_channels}, 1, H, W], got {tuple(sample.shape)}")
+        if sample.dtype not in (torch.float16, torch.float32):
+            raise TypeError("sample must be fp16 or fp32")
+        if not 0 <= int(up_ft_index) <= 3:
+            raise ValueError(f"up_ft_index must be in 0..3, got {up_ft_index}")
+        N, _, _, H, W = sample.shape
+        if encoder_hidden_states.dim() != 3 or encoder_hidden_states.shape[0] != N or \
+                encoder_hidden_states.shape[-1] != self.cfg.cross_attention_dim:
+            raise ValueError(f"encoder_hidden_states must be [{N}, tokens, {self.cfg.cross_attention_dim}], got "
+                             f"{tuple(encoder_hidden_states.shape)}")
+        dev = sample.device
+        k = int(up_ft_index)
+        lh, lw = self.level_sizes(H, W)[2 - k] if k < 3 else (H, W)
+        ck = self.cfg.block_out_channels[3 - k]
+        with torch.cuda.device(dev):
+            self._sync_weights(dev)
+            x = sample.contiguous()
+            if torch.is_tensor(timestep):
+                t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
+            else:
+                t = torch.tensor([float(timestep)], dtype=torch.float32, device=dev)
+            t = t.expand(N).contiguous()
+            ehs = encoder_hidden_states.to(device=dev, dtype=torch.float16).contiguous()
+            out = torch.empty((N, lh, lw, ck), dtype=torch.float16, device=dev)
+            _lib.call("vs_unet_forward_features", self._handle, torch.cuda.current_stream().cuda_stream, x.data_ptr(),
+                      int(x.dtype == torch.float32), N, 1, H, W, t.data_ptr(), ehs.data_ptr(), ehs.shape[1], 0, k,
+                      out.data_ptr())
+            self._keepalive = (x, t, ehs)
+        return out
+
+
 UNet3DConditionModel = AnimateDiffUNet3DModel
