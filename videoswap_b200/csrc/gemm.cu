@@ -29,7 +29,7 @@
 // Epilogue (per consumer warp, 16 rows of each 64-row half, one half after the other): registers -> [folded LayerNorm:
 // rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU / quick-GELU -> fp16 -> warp-private
 // swizzled shared-memory transpose, 32 columns at a time -> (+ fp16 residual) -> coalesced 16-byte global stores.
-// Tiny-N outputs (conv_out, N = 4) keep a direct-store path.
+// Tiny-N or unaligned outputs (conv_out, N = 4) keep a direct-store path with the same rounding order.
 //
 // Replaces (reference call sites): InflatedConv3d 3x3 / 1x1 (models/animatediff_models/resnet.py:9-18), every
 // nn.Linear / 1x1 conv of Transformer3DModel (attention.py:65-93,174-204) and the motion module
@@ -454,8 +454,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
               float f = acc[hh][4 * j + e];
               if (has_bias) f += p.bias[n];
               if (rv[h]) f += rv[h][c];
-              if (p.residual) f += __half2float(p.residual[(long long)pix[h] * p.ldr + n]);
-              p.out[(long long)pix[h] * p.ldc + n] = __float2half_rn(f);
+              __half y = __float2half_rn(f);
+              if (p.residual) y = __hadd(y, p.residual[(long long)pix[h] * p.ldr + n]);   // fp16 add, as the staged path
+              p.out[(long long)pix[h] * p.ldc + n] = y;
             }
           }
         }
