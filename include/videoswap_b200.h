@@ -81,6 +81,11 @@ int vs_unet_forward(vs_unet* h, void* stream, const void* d_sample, int io_f32, 
 int vs_unet_forward_features(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W,
                              const float* d_timesteps, const void* d_ehs, int ehs_tokens, int ehs_layers, int up_ft_index,
                              void* d_feat);
+/* The time embedding exactly as vs_unet_forward runs it, with the handle's loaded weights: d_timesteps fp32 [B] ->
+ * d_emb fp32 [B, 4 block_out_channels[0]] (time_embedding(Timesteps(t))) and d_proj fp32 [B, tproj_n], every resnet's
+ * time_emb_proj(SiLU(emb)) side by side in registration order (down blocks, mid block, up blocks; tproj_n is the sum of
+ * their output channels).  Uses neither the workspace nor a captured graph's buffers. */
+int vs_unet_time_embedding(vs_unet* h, void* stream, const float* d_timesteps, int B, float* d_emb, float* d_proj);
 size_t vs_unet_workspace_bytes(const vs_unet* h);
 /* The activation workspace is one arena that only grows: a forward of a smaller shape re-uses it.  A captured CUDA graph
  * holds raw pointers into it, so the owner of a graph pins the arena (pin != 0; unpin with 0 when the graph dies): while

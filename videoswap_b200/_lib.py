@@ -67,6 +67,7 @@ _SIGNATURES = {
     "vs_unet_num_params": (_I, [_P]),
     "vs_unet_param_name": (C.c_char_p, [_P, _I]),
     "vs_unet_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _I, C.POINTER(_P), _I, _F, _P]),
+    "vs_unet_time_embedding": (_I, [_P, _P, _P, _I, _P, _P]),
     "vs_unet_workspace_bytes": (_SZ, [_P]),
     "vs_unet_pin_workspace": (_I, [_P, _I]),
     "vs_unet_reserve_workspace": (_I, [_P, _I, _I, _I, _I]),

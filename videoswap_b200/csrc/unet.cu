@@ -742,6 +742,19 @@ extern "C" int vs_unet_copy_tap(const vs_unet* h, void* stream, int i, void* d_d
 
 namespace {
 
+// Time embedding (unet.py:376-397): Timesteps -> Linear -> SiLU -> Linear into emb [B, temb]; then every resnet's
+// projection of SiLU(emb) in one stacked tiny-M linear (resnet.py:171-172) into proj [B, tproj_n], resnet r at column
+// r.temb_off.  te0 [B, boc0] and te1 [B, temb] are scratch.
+int time_embedding(const vs_unet* h, cudaStream_t st, const float* d_t, int B, float* te0, float* te1, float* emb,
+                   float* proj) {
+  const int c0 = h->cfg.block_out_channels[0], temb = c0 * 4;
+  RUN(timestep_embedding(st, d_t, B, c0, te0));
+  RUN(small_linear(st, te0, B, c0, h->te1.w, h->te1.b, temb, false, true, te1));
+  RUN(small_linear(st, te1, B, temb, h->te2.w, h->te2.b, temb, false, false, emb));
+  RUN(small_linear(st, emb, B, temb, h->tproj_w, h->tproj_b, h->tproj_n, true, false, proj));
+  return 0;
+}
+
 // The body of vs_unet_forward.  stop_up >= 0 (vs_unet_forward_features) runs the 2-D UNet: no motion module, and the walk
 // ends after up block `stop_up` (with its up-sampler), whose output is copied to d_out as NHWC fp16.
 int unet_run(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, int F, int H, int W, const float* d_timesteps,
@@ -777,12 +790,7 @@ int unet_run(vs_unet* h, void* stream, const void* d_sample, int io_f32, int B, 
   Ctx c{h, st, B, F, B * F, H, W, (const __half*)d_ehs, ehs_tokens, ehs_layers};
 
   VS_CHECK_CUDA(cudaMemsetAsync(h->F_SUMS, 0, (size_t)h->n_groupnorms * c.NI * 64 * sizeof(float), st));
-  // ---- time embedding (unet.py:376-397): Timesteps -> Linear -> SiLU -> Linear; then every resnet's projection of
-  //      SiLU(emb) in one stacked tiny-M linear (resnet.py:171-172)
-  RUN(timestep_embedding(st, d_timesteps, B, boc[0], h->F_TE0));
-  RUN(small_linear(st, h->F_TE0, B, boc[0], h->te1.w, h->te1.b, temb, false, true, h->F_TE1));
-  RUN(small_linear(st, h->F_TE1, B, temb, h->te2.w, h->te2.b, temb, false, false, h->F_EMB));
-  RUN(small_linear(st, h->F_EMB, B, temb, h->tproj_w, h->tproj_b, h->tproj_n, true, false, h->F_TPROJ));
+  RUN(time_embedding(h, st, d_timesteps, B, h->F_TE0, h->F_TE1, h->F_EMB, h->F_TPROJ));
 
   // ---- conv_in
   RUN(ncfhw_to_nhwc(st, d_sample, io_f32, B, cf.in_channels, F, H, W, h->XIN));
@@ -931,4 +939,15 @@ extern "C" int vs_unet_forward_features(vs_unet* h, void* stream, const void* d_
   VS_REQUIRE(h->hook == nullptr, "vs_unet_forward_features: the featurizer runs without attention controllers (a hook is set)");
   return unet_run(h, stream, d_sample, io_f32, B, F, H, W, d_timesteps, d_ehs, ehs_tokens, ehs_layers, nullptr, 0, 1.f,
                   up_ft_index, d_feat);
+}
+
+extern "C" int vs_unet_time_embedding(vs_unet* h, void* stream, const float* d_timesteps, int B, float* d_emb, float* d_proj) {
+  VS_REQUIRE(h && d_timesteps && d_emb && d_proj, "vs_unet_time_embedding: null argument");
+  VS_REQUIRE(B >= 1, "vs_unet_time_embedding: bad batch %d", B);
+  const int c0 = h->cfg.block_out_channels[0];
+  // the sinusoid and the first hidden layer live in d_proj until the last launch, which reads only d_emb, overwrites them
+  VS_REQUIRE(h->tproj_n >= 5 * c0, "vs_unet_time_embedding: projections too narrow to hold the scratch rows");
+  float* te0 = d_proj;
+  float* te1 = d_proj + (size_t)B * c0;
+  return time_embedding(h, (cudaStream_t)stream, d_timesteps, B, te0, te1, d_emb, d_proj);
 }

@@ -616,5 +616,24 @@ class AnimateDiffUNet3DModel(nn.Module):
             self._keepalive = (x, t, ehs)
         return out
 
+    @torch.no_grad()
+    def time_embedding_rows(self, timesteps: torch.Tensor):
+        """The forward's time embedding for timesteps [B] -> (emb fp32 [B, time_embed_dim], proj fp32 [B, tproj_n]): proj
+        holds every resnet's time_emb_proj(SiLU(emb)) side by side, in the order the library registers the resnets."""
+        dev = self.conv_in.weight.device
+        if dev.type != "cuda":
+            raise RuntimeError("AnimateDiffUNet3DModel (videoswap_b200) runs on CUDA only: there is no CPU path")
+        tproj_n = sum(m.time_emb_proj.weight.shape[0] for m in self.modules() if isinstance(getattr(m, "time_emb_proj", None), _Holder))
+        with torch.cuda.device(dev):
+            self._sync_weights(dev)
+            t = timesteps.to(device=dev, dtype=torch.float32).reshape(-1).contiguous()
+            B = t.numel()
+            emb = torch.empty((B, self.cfg.time_embed_dim), dtype=torch.float32, device=dev)
+            proj = torch.empty((B, tproj_n), dtype=torch.float32, device=dev)
+            _lib.call("vs_unet_time_embedding", self._handle, torch.cuda.current_stream().cuda_stream, t.data_ptr(), B,
+                      emb.data_ptr(), proj.data_ptr())
+            self._keepalive = (t,)
+        return emb, proj
+
 
 UNet3DConditionModel = AnimateDiffUNet3DModel
