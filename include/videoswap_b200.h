@@ -351,6 +351,8 @@ int vs_profile_dump(const char* path);   /* CSV: category, shape (m,n,k), work p
  *   "gemm_stages"  0  limit of the shared-memory ring depth of the GEMM (0 = as many as fit)
  *   "gemm_ctas"    0  cap on the persistent grid of the GEMM (0 = one CTA per SM); a smaller grid gives every CTA more
  *                     tiles, so the same problem runs another tile schedule (schedule-invariance tests)
+ *   "gemm_epi_slot" 1 the short-K linears and GEGLUs (K <= 640) fetch their epilogue operands into shared-memory slots
+ *                     during the main loop; 0 = the epilogue reads them from global memory (bit-identical; tests)
  *   "ln_fold"      1  LayerNorms folded into the consuming GEMM; 0 = stand-alone LayerNorm kernel
  *   "ln_fuse"      1  row statistics of folded LayerNorms written by the producing GEMM's epilogue; 0 = ln_stats pass
  *   "tattn_vst"    1  temporal attention writes its outputs with 16-byte stores from a shared-memory stage; 0 = 4-byte stores

@@ -30,6 +30,9 @@
 // rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU / quick-GELU -> fp16 -> warp-private
 // swizzled shared-memory transpose, 32 columns at a time -> (+ fp16 residual) -> coalesced 16-byte global stores.
 // Tiny-N or unaligned outputs (conv_out, N = 4) keep a direct-store path with the same rounding order.
+// The short-K linears (K <= 640, BN 128 / 160) and GEGLUs (K <= 640, BN 256; GemmParamsEpi) read no global memory in the
+// epilogue: warp 1 of the producer warpgroup fetches each tile's bias / LayerNorm / row-vector / residual operands into
+// one of two shared-memory slots while the tile's main loop runs (see EpiSlot).
 //
 // Replaces (reference call sites): InflatedConv3d 3x3 / 1x1 (models/animatediff_models/resnet.py:9-18), every
 // nn.Linear / 1x1 conv of Transformer3DModel (attention.py:65-93,174-204) and the motion module
@@ -105,7 +108,29 @@ struct GemmParamsS2 : GemmParams {
   CUtensorMap tmP[3];
 };
 
-template <int BN>
+// Short-K linears and GEGLUs (GemmParamsEpi): the producer warpgroup's second warp fetches each tile's epilogue operands
+// into a shared-memory slot while the tile's main loop runs; the epilogue then reads shared memory only.  Two slots, each
+// guarded by its own full / empty mbarrier pair; tile j of a CTA uses slot j % 2 (ping-pong: the slot of the consumer
+// that takes the tile; cooperative GEGLU: both consumers read it, so the next tile's slot fills during this epilogue).
+constexpr int LN_MAX_PARTS = 8;                     // LayerNorm partial-sum slices a slot holds
+struct GemmParamsEpi : GemmParams {
+  CUtensorMap tmR;   // residual [M, N] fp16: boxes of 32 columns x 128 rows, 64-byte swizzle (= the epilogue's sw64_off)
+};
+
+template <int BN, int EPI>
+struct EpiSlot {
+  static constexpr bool RES = (EPI & EPI_F_RES) != 0, LN = (EPI & EPI_F_LN) != 0, RV = (EPI & EPI_F_RV) != 0;
+  static constexpr int RES_BYTES = RES ? BM * BN * 2 : 0;              // BN / 32 boxes of [128 rows x 64 B], first
+  static constexpr int BIAS_OFF = RES_BYTES;                           // bias[n0, n0 + BN)
+  static constexpr int U_OFF = BIAS_OFF + BN * 4;                      // LN: ln_u[n0, n0 + BN)
+  static constexpr int RV_OFF = U_OFF + (LN ? BN * 4 : 0);             // RV: the (at most 2) row-vector rows of the tile
+  static constexpr int LNR_OFF = RV_OFF + (RV ? 2 * BN * 4 : 0);       // LN: [parts][128 rows] float2 row statistics
+  static constexpr int END = LNR_OFF + (LN ? LN_MAX_PARTS * BM * 8 : 0);
+  // the residual's swizzle repeats every 512 B, so a slot that holds one starts 1024-aligned
+  static constexpr int BYTES = RES ? (END + 1023) / 1024 * 1024 : (END + 127) / 128 * 128;
+};
+
+template <int BN, int SLOT_BYTES = 0>
 struct Cfg {
   // Cooperative (both consumers on one 128 x BN tile, 64 rows each) for BN = 256: 128 accumulators a thread.  Ping-pong
   // (one consumer owns the whole tile: two m64 halves, BN accumulators a thread) for the narrower tiles.
@@ -113,11 +138,15 @@ struct Cfg {
   static constexpr int HALVES = COOP ? 1 : 2;       // 64-row accumulator halves per consumer
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
+  // with epilogue slots the ring gets what the two slots leave (counted without the spare kilobyte of the others)
+  static constexpr int STAGES_RAW = SLOT_BYTES ? (SMEM_LIMIT - 1024 - 256 - EPI_BYTES - 2 * SLOT_BYTES) / STAGE_BYTES
+                                               : (SMEM_LIMIT - 2048 - EPI_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 12 ? 12 : STAGES_RAW;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES =
+      STAGES * STAGE_BYTES + EPI_BYTES + 2 * SLOT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(B_STAGE_BYTES % 1024 == 0, "B stage must keep 1024-byte alignment for SWIZZLE_128B");
   static_assert(STAGES >= 3, "pipeline too shallow");
+  static_assert(SMEM_BYTES <= SMEM_LIMIT, "shared memory");
   static_assert(BN % 32 == 0 && BN <= 256, "wgmma N");
 };
 
@@ -127,9 +156,12 @@ __device__ __forceinline__ uint32_t sw64_off(int row, int chunk) {   // byte off
 
 template <int BN, int EPI, typename Params>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ Params p) {
-  using C = Cfg<BN>;
   constexpr bool SUB = std::is_same<Params, GemmParamsSub>::value;
   constexpr bool S2 = std::is_same<Params, GemmParamsS2>::value;
+  constexpr bool SLOT = std::is_same<Params, GemmParamsEpi>::value;   // epilogue operands through the slots
+  using ES = EpiSlot<BN, EPI>;
+  using C = Cfg<BN, SLOT ? ES::BYTES : 0>;
+  static_assert(!SLOT || ((C::COOP == ((EPI & EPI_F_GEGLU) != 0)) && (EPI & EPI_F_QGELU) == 0), "epilogue slots: ping-pong linears and cooperative GEGLUs");
   constexpr bool GEGLU = (EPI & EPI_F_GEGLU) != 0, HAS_RES = (EPI & EPI_F_RES) != 0, HAS_RV = (EPI & EPI_F_RV) != 0;
   // LN: the A operand is the RAW input of a LayerNorm whose affine map is folded into the weights:
   //   LN(x) W^T = rstd (x W'^T) - rstd mean u + c,  W' = W * gamma, u[n] = sum_k W'[n,k], c = beta W^T + bias (the `bias`)
@@ -143,10 +175,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t epi_base = smem_base + C::STAGES * C::STAGE_BYTES;
-  const uint32_t bar_base = epi_base + EPI_BYTES;
-  // barrier layout: full[S], empty[S]
+  const uint32_t slot_base = epi_base + EPI_BYTES;   // SLOT: consumer g's slot at slot_base + g * ES::BYTES
+  const uint32_t bar_base = slot_base + (SLOT ? 2 * ES::BYTES : 0);
+  // barrier layout: full[S], empty[S], SLOT: slot_full[2], slot_empty[2]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
+  auto slot_full = [&](int g) { return bar_base + 8u * (2 * C::STAGES + g); };
+  auto slot_empty = [&](int g) { return bar_base + 8u * (2 * C::STAGES + 2 + g); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -168,6 +203,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     if constexpr (S2) {
       for (int k = 0; k < 3; ++k) prefetch_tmap(&p.tmP[k]);
     }
+    if constexpr (SLOT) {
+      if (ES::RES) prefetch_tmap(&p.tmR);
+      for (int g = 0; g < 2; ++g) {
+        mbar_init(slot_full(g), 1);
+        mbar_init(slot_empty(g), C::COOP ? 8 : 4);   // one arrival per warp of the consumer(s) that read the slot
+      }
+    }
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), C::COOP ? 8 : 4);  // one arrival per warp of the consumer(s) that read the stage
@@ -180,6 +222,54 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 
   if (wg == 0) {
     setmaxnreg_dec<PRODUCER_REGS>();
+    if constexpr (SLOT) {
+      if (warp == 1) {
+        // ================================================================= epilogue-operand loader (one elected issuer)
+        // Fills slot g = j % 2 for tile j of the CTA as soon as the epilogue of tile j - 2 has released it, so the
+        // copies land during tile j's main loop (ping-pong: while consumer g waits for the tensor cores and runs it;
+        // cooperative: during the epilogue of tile j - 1 and tile j's main loop).  In-place residual (residual == out): a tile's residual block is read here, by this
+        // tile only, before its own epilogue writes it; no other tile writes those rows and columns.
+        for (int t = blockIdx.x, j = 0; t < total_tiles; t += gridDim.x, ++j) {
+          const int g = j & 1;
+          mbar_wait(slot_empty(g), ((j >> 1) & 1) ^ 1);
+          if (elect_one()) {
+            const int m_tile = t / p.n_tiles, n_tile = t % p.n_tiles;
+            const int n0 = n_tile * BN, m0 = m_tile * BM;
+            const int ncols = p.N - n0 < BN ? p.N - n0 : BN;      // a multiple of 32 (staged epilogue)
+            const int parts = p.ln_nparts > 0 ? p.ln_nparts : 1;
+            const int rows = p.M - m0 < BM ? p.M - m0 : BM;       // even (the host requires an even M for LN)
+            // row-vector rows of the tile's first and last row (the host allows at most two per tile)
+            const int last = m0 + rows - 1;
+            int rv0 = m0 / p.pix_per_batch, rv1 = last / p.pix_per_batch;
+            const int nrv = rv1 != rv0 ? 2 : 1;
+            if (p.rv_mod > 0) { rv0 %= p.rv_mod; rv1 %= p.rv_mod; }
+            const uint32_t sb = slot_base + (uint32_t)g * ES::BYTES, fb = slot_full(g);
+            uint32_t bytes = p.bias != nullptr ? ncols * 4u : 0u;
+            if (ES::RES) bytes += (uint32_t)(ncols / EPI_COLS) * (BM * 64);
+            if (ES::LN) bytes += ncols * 4u + (uint32_t)(parts * rows) * 8u;
+            if (ES::RV) bytes += (uint32_t)nrv * ncols * 4u;
+            mbar_expect_tx(fb, bytes);
+            if (p.bias != nullptr) bulk_load(sb + ES::BIAS_OFF, p.bias + n0, ncols * 4u, fb);
+            if constexpr (ES::RES) {
+              for (int c = 0; c < ncols / EPI_COLS; ++c) tma_load_2d(sb + c * (BM * 64), &p.tmR, fb, n0 + c * EPI_COLS, m0);
+            }
+            if constexpr (ES::LN) {
+              bulk_load(sb + ES::U_OFF, p.ln_u + n0, ncols * 4u, fb);
+              // the tile's rows of each slice; slot rows past M keep stale values and are never stored
+              const float2* src = p.ln_nparts > 0 ? p.ln_parts : p.ln_stats;
+              for (int k = 0; k < parts; ++k)
+                bulk_load(sb + ES::LNR_OFF + k * (BM * 8), src + (long long)k * p.M + m0, rows * 8u, fb);
+            }
+            if constexpr (ES::RV) {
+              bulk_load(sb + ES::RV_OFF, p.rowvec + (long long)rv0 * p.ldrv + n0, ncols * 4u, fb);
+              if (nrv == 2) bulk_load(sb + ES::RV_OFF + BN * 4, p.rowvec + (long long)rv1 * p.ldrv + n0, ncols * 4u, fb);
+            }
+          }
+          __syncwarp();
+        }
+        return;
+      }
+    }
     if (warp != 0) return;
     // =================================================================== TMA producer (whole warp, one elected issuer)
     const int num_kb = p.num_kb, kb_per_tap = p.kb_per_tap, kb_src1 = p.kb_src1;
@@ -245,7 +335,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   const int rbase = 16 * wq + (lane >> 2);     // this thread's rows of a half: rbase and rbase + 8
   const uint32_t stage_buf = epi_base + (uint32_t)(warp - 4) * EPI_WARP_BYTES;
   const bool has_bias = p.bias != nullptr;
-  const bool staged = p.staged != 0;
+  const bool staged = SLOT || p.staged != 0;
   const int num_kb = p.num_kb;
   // output pixel (row of the GEMM) of tile row `row`, -1 = outside the problem
   auto tile_pixel = [&](int m_tile, int row) -> int {
@@ -305,6 +395,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     if (!C::COOP && t + (int)gridDim.x < total_tiles) named_bar_arrive(bar_other, 256);
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(empty_bar(prev));
+    // SLOT: this tile's epilogue operands, read through a generic pointer into the slot (plain shared loads the compiler
+    // may schedule freely; the slot is written only by the async proxy, ordered by the mbarrier waits and arrivals)
+    const int js = j & 1;                       // this tile's slot (ping-pong: js == g)
+    const uint8_t* slot = smem_raw + (slot_base + (uint32_t)js * ES::BYTES - smem_u32(smem_raw));
+    if constexpr (SLOT) mbar_wait(slot_full(js), (uint32_t)(j >> 1) & 1u);
 
     // ------------------------------------------------------------------ epilogue, one 64-row half at a time
     const int n0 = n_tile * BN;
@@ -315,7 +410,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       pix[0] = tile_pixel(m_tile, r0);
       pix[1] = tile_pixel(m_tile, r0 + 8);
       const float* rv[2] = {nullptr, nullptr};
-      if (HAS_RV || !staged) {
+      if (SLOT && HAS_RV) {                    // row h's row vector: the slot's first or second row
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int d = pix[h] >= 0 ? pix[h] / p.pix_per_batch - (m_tile * BM) / p.pix_per_batch : 0;
+          rv[h] = reinterpret_cast<const float*>(slot + ES::RV_OFF) + d * BN;
+        }
+      } else if (HAS_RV || !staged) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (p.rowvec != nullptr && pix[h] >= 0) {
@@ -334,17 +435,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (pix[h] < 0) continue;
+            const float2* lnr = reinterpret_cast<const float2*>(slot + ES::LNR_OFF) + r0 + 8 * h;   // SLOT: [parts][128]
             if (p.ln_nparts > 0) {            // statistics from the producer GEMM's per-column-tile partial sums
               float S = 0.f, Q = 0.f;
               for (int k = 0; k < p.ln_nparts; ++k) {
-                const float2 v = __ldg(p.ln_parts + (long long)k * p.M + pix[h]);
+                const float2 v = SLOT ? lnr[k * BM] : __ldg(p.ln_parts + (long long)k * p.M + pix[h]);
                 S += v.x; Q += v.y;
               }
               const float mean = S * p.ln_inv_c;
               la[h] = rsqrtf(fmaxf(fmaf(-mean, mean, Q * p.ln_inv_c), 0.f) + 1e-5f);
               lb[h] = -mean * la[h];
             } else {
-              const float2 st2 = __ldg(p.ln_stats + pix[h]);
+              const float2 st2 = SLOT ? lnr[0] : __ldg(p.ln_stats + pix[h]);
               la[h] = st2.x; lb[h] = st2.y;
             }
           }
@@ -363,7 +465,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         for (int sb = 0; sb < OC / EPI_COLS; ++sb) {
           if (sb >= nsub) break;                  // warp-uniform
           uint4 rr[2];
-          if (HAS_RES) {
+          if (SLOT && HAS_RES) {                  // box sb of the slot, 64-byte swizzled as the staging buffer
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              rr[h] = *reinterpret_cast<const uint4*>(slot + sb * (BM * 64) + sw64_off(r0 + 8 * h, q));
+          } else if (HAS_RES) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) rr[h] = __ldg(reinterpret_cast<const uint4*>(rrow[h] + sb * EPI_COLS));
           }
@@ -371,12 +477,23 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
           for (int jj = 0; jj < 4; ++jj) {
             const int j = 4 * sb + jj;            // n8 block of the (output) tile
             const int c = 8 * j + 2 * q;          // column inside the tile (value column for GEGLU)
-            float2 b = has_bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
-            float2 u = LN ? __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + c)) : make_float2(0.f, 0.f);
+            float2 b = make_float2(0.f, 0.f), u = make_float2(0.f, 0.f);
+            if constexpr (SLOT) {
+              if (has_bias) b = *reinterpret_cast<const float2*>(slot + ES::BIAS_OFF + 4 * c);
+              if (LN) u = *reinterpret_cast<const float2*>(slot + ES::U_OFF + 4 * c);
+            } else {
+              if (has_bias) b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
+              if (LN) u = __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + c));
+            }
             float2 bg = make_float2(0.f, 0.f), ug = make_float2(0.f, 0.f);
             if (GEGLU) {                          // gate columns are BN / 2 further on, in the same thread's registers
-              bg = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + BN / 2 + c));
-              if (LN) ug = __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + BN / 2 + c));
+              if constexpr (SLOT) {
+                bg = *reinterpret_cast<const float2*>(slot + ES::BIAS_OFF + 4 * (BN / 2 + c));
+                if (LN) ug = *reinterpret_cast<const float2*>(slot + ES::U_OFF + 4 * (BN / 2 + c));
+              } else {
+                bg = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + BN / 2 + c));
+                if (LN) ug = __ldg(reinterpret_cast<const float2*>(p.ln_u + n0 + BN / 2 + c));
+              }
             }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -399,7 +516,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                   f0 += b.x; f1 += b.y;
                 }
                 if (HAS_RV && rv[h] != nullptr) {
-                  const float2 r2 = __ldg(reinterpret_cast<const float2*>(rv[h] + c));
+                  const float2 r2 = SLOT ? *reinterpret_cast<const float2*>(rv[h] + c)
+                                         : __ldg(reinterpret_cast<const float2*>(rv[h] + c));
                   f0 += r2.x; f1 += r2.y;
                 }
                 if constexpr (QGELU) {
@@ -407,8 +525,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 }
               }
               const __half2 hv = __floats2half2_rn(f0, f1);
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(stage_buf + sw64_off((lane >> 2) + 8 * h, jj) + 4 * q),
-                           "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
+              const uint32_t sa = stage_buf + sw64_off((lane >> 2) + 8 * h, jj) + 4 * q;
+              if constexpr (SLOT)                 // no global loads to order against; the volatile asms keep their order
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(sa), "r"(*reinterpret_cast<const uint32_t*>(&hv)));
+              else
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(sa), "r"(*reinterpret_cast<const uint32_t*>(&hv)) : "memory");
             }
           }
           __syncwarp();
@@ -462,6 +583,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
         }
       }
     }
+    if constexpr (SLOT) {                      // every slot value this warp read has gone into a store: release the slot
+      __syncwarp();
+      if (lane == 0) mbar_arrive(slot_empty(js));
+    }
   }
 }
 
@@ -486,7 +611,7 @@ ConvTile pick_conv_tile(int nimg, int H, int W) {   // BM pixels as a TW x TH x 
 
 template <int BN, int EPI, typename Params = GemmParams>
 int launch(cudaStream_t st, const Params& p) {
-  using C = Cfg<BN>;
+  using C = Cfg<BN, std::is_same<Params, GemmParamsEpi>::value ? EpiSlot<BN, EPI>::BYTES : 0>;
   static bool configured = false;
   if (!configured) {
     VS_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI, Params>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
@@ -513,6 +638,50 @@ int launch_linear(cudaStream_t st, const GemmParams& p) {
     case EPI_F_RV: return launch<BN, EPI_F_RV>(st, p);
     case EPI_F_RES | EPI_F_RV: return launch<BN, EPI_F_RES | EPI_F_RV>(st, p);
     default: set_error("gemm_tc: unsupported epilogue combination 0x%x", epi); return 2;
+  }
+}
+
+// The epilogue-slot launches (GemmParamsEpi); -1 = this launch keeps the parameter block without slots.
+// K <= 640 (10 k-blocks); the staged epilogue of a plain linear on a ping-pong tile with one of the transformer's
+// epilogue combinations, or of a GEGLU (BN 256, cooperative); operands the bulk copies can fetch: 16-byte aligned
+// LayerNorm rows (an even M, so every slice and every tile's rows start 16-byte aligned and span a multiple of 16 bytes)
+// of at most LN_MAX_PARTS slices, and at most two row-vector rows per 128-row tile.
+template <int BN>
+int launch_linear_slot(cudaStream_t st, const GemmParams& p, const GemmArgs& a) {
+  const bool geglu = a.mode == EPI_GEGLU;
+  if (get_option("gemm_epi_slot") == 0 || a.taps != 1 || (a.mode != EPI_LINEAR && !geglu) || !p.staged || p.num_kb > 10)
+    return -1;
+  const int epi = (p.residual ? EPI_F_RES : 0) | (p.rowvec ? EPI_F_RV : 0) | ((p.ln_stats || p.ln_parts) ? EPI_F_LN : 0) |
+                  (p.ln_sums_out ? EPI_F_LNOUT : 0) | (geglu ? EPI_F_GEGLU : 0);
+  if (geglu ? (BN != 256 || (epi & ~EPI_F_LN) != EPI_F_GEGLU)
+            : (BN == 256 || (epi != EPI_F_RES && epi != EPI_F_LNOUT && epi != (EPI_F_LNOUT | EPI_F_RES) &&
+                             epi != EPI_F_LN && epi != (EPI_F_LN | EPI_F_RV))))
+    return -1;
+  GemmParamsEpi pe;
+  memset(&pe, 0, sizeof(pe));
+  static_cast<GemmParams&>(pe) = p;
+  if (p.rowvec && !(p.pix_per_batch >= BM || p.pix_per_batch == BM / 2)) return -1;
+  if (epi & EPI_F_LN) {
+    const void* rows = p.ln_parts ? static_cast<const void*>(p.ln_parts) : static_cast<const void*>(p.ln_stats);
+    const int parts = p.ln_parts ? p.ln_nparts : 1;
+    if (parts > LN_MAX_PARTS || (reinterpret_cast<uintptr_t>(rows) & 15) != 0 || (p.M & 1) != 0) return -1;
+  }
+  if (epi & EPI_F_RES) {
+    const uint64_t dims[2] = {(uint64_t)p.N, (uint64_t)p.M};
+    const uint64_t str[1] = {(uint64_t)p.ldr * 2};
+    const uint32_t box[2] = {EPI_COLS, BM};
+    if (make_tmap_f16(&pe.tmR, p.residual, 2, dims, str, box, 2)) return 3;
+  }
+  if constexpr (BN == 256) {
+    return epi == EPI_F_GEGLU ? launch<BN, EPI_F_GEGLU>(st, pe) : launch<BN, EPI_F_GEGLU | EPI_F_LN>(st, pe);
+  } else {
+    switch (epi) {
+      case EPI_F_RES: return launch<BN, EPI_F_RES>(st, pe);
+      case EPI_F_LNOUT: return launch<BN, EPI_F_LNOUT>(st, pe);
+      case EPI_F_LNOUT | EPI_F_RES: return launch<BN, EPI_F_LNOUT | EPI_F_RES>(st, pe);
+      case EPI_F_LN: return launch<BN, EPI_F_LN>(st, pe);
+      default: return launch<BN, EPI_F_LN | EPI_F_RV>(st, pe);
+    }
   }
 }
 
@@ -699,6 +868,7 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
   if (a.ln_sums_out) VS_REQUIRE(p.staged, "gemm_tc: row statistics output needs the staged epilogue (N %% 32 == 0, aligned rows)");
   ProfScope prof(st, a.taps != 1 ? PC_CONV : PC_GEMM, 2.0 * a.M * (double)a.N * Ktot, 1, a.M, a.N, Ktot);
   if (a.mode == EPI_GEGLU) {
+    if (const int e = launch_linear_slot<256>(st, p, a); e >= 0) return e;
     if (p.ln_stats || p.ln_parts) return launch<256, EPI_F_GEGLU | EPI_F_LN>(st, p);
     return launch<256, EPI_F_GEGLU>(st, p);
   }
@@ -722,6 +892,10 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
       case 256: return launch<256, 0, GemmParamsSub>(st, ps);
       default: return launch<160, 0, GemmParamsSub>(st, ps);
     }
+  }
+  if (bn == 128 || bn == 160) {
+    const int e = bn == 128 ? launch_linear_slot<128>(st, p, a) : launch_linear_slot<160>(st, p, a);
+    if (e >= 0) return e;
   }
   switch (bn) {
     case 64: return launch_linear<64>(st, p);

@@ -117,7 +117,8 @@ struct Option { const char* name; int value; };
 static Option g_options[] = {
     {"attn_tc", 1},        // wgmma attention for d = 40 / 80 (0 = mma.sync kernel)
     {"gemm_stages", 0},    // smem ring depth limit (0 = all)
-    {"gemm_ctas", 0},      // persistent GEMM grid cap (0 = one CTA per SM); tests run other tile schedules with it
+    {"gemm_ctas", 0},
+    {"gemm_epi_slot", 1},  // short-K linears and GEGLUs read their epilogue operands from shared-memory slots (0 = from global memory)      // persistent GEMM grid cap (0 = one CTA per SM); tests run other tile schedules with it
     {"ln_fold", 1},        // LayerNorms folded into the GEMM that consumes them (0 = stand-alone LayerNorm kernel)
     {"ln_fuse", 1},        // row statistics of folded LayerNorms come from the producing GEMM's epilogue (0 = ln_stats_kernel pass)
     {"tattn_vst", 1},      // temporal attention: outputs staged in shared memory and written with 16-byte stores (0 = 4-byte)
