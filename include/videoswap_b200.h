@@ -337,6 +337,41 @@ int vs_dift_ensemble_mean(void* stream, const void* d_feat, int n, int E, int h,
 int vs_dift_point_reduce(void* stream, const float* d_vecs, int n, int P, int C, const float* d_src, const int* d_src_row,
                          float* d_conf, const void* d_accept, float* d_sums, float* d_counts, float* d_means);
 
+/* ---- layered-atlas point propagation (the reference's propagate_point_displacement.py) ---------------------------------
+ * One IMLP_Hash network with mlp_type 'origin' (videoswap/atlas/implicit_neural_networks.py): the positional encoding
+ * (pe_dim 0 = pe_type 'none'; pe_dim > 0 = 'encoding', feature j (2 input_dim) + c = sin(x_c b_j) for c < input_dim and
+ * cos(x_(c - input_dim) b_j) after, b_j = fp32(2^j pi)), then mlp_layers linears with a ReLU before every one but the first;
+ * layer i with bit i of skip_mask set takes torch.cat((x, encoded input), 1); tanh on the output when use_tanh.
+ * d_params: fp32, 16-byte aligned, for each layer i in order W_i^T [K_i, N_i] (the transposed nn.Linear weight) then the
+ * bias [N_i]; K_0 = E (the encoded width: input_dim, or 2 input_dim pe_dim), K_i = hidden_dim (+ E with the skip bit),
+ * N_i = hidden_dim except N_(mlp_layers - 1) = output_dim.  fp32 FMA on the CUDA cores. */
+typedef struct vs_imlp_desc {
+  const float* d_params;
+  int input_dim;      /* 1 .. 8 */
+  int output_dim;     /* 1 .. hidden_dim */
+  int hidden_dim;     /* 32 .. 256, a multiple of 32 */
+  int mlp_layers;     /* 1 .. 32 */
+  int pe_dim;         /* 0 .. 16 */
+  uint32_t skip_mask; /* bits 1 .. mlp_layers - 1 only */
+  int use_tanh;
+} vs_imlp_desc;
+/* d_out fp32 [rows, output_dim] = the network on d_x fp32 [rows, input_dim], rows >= 1, in one launch.  A descriptor
+ * outside the ranges above (or one whose encoded width does not fit the row tile's shared memory) fails before any launch. */
+int vs_imlp_forward(void* stream, const vs_imlp_desc* net, const float* d_x, int rows, float* d_out);
+/* propagate_point_sequence for P edited points over F frames in six launches, whatever P and F, with no host sync.
+ * fg (3 -> 2), fg_inverse (3 -> 3), alpha (3 -> 1): FG_UV_Mapping, FG_UV_Mapping_Inverse and F_Alpha.
+ * d_points fp32 [P, 4] = (x, y, dx, dy): the keyframe point and the drag, normalised as x / (larger_dim / 2) - 1 (the drag as
+ * the difference of two normalised coordinates); t_key the normalised keyframe time.  The frame axis is
+ * fp32(f) / fp32(F / 2) - 1 in fp32.  d_tracks fp32 [F, P, 2] = (x, y) pixels, rint((w + 1) / 2 larger_dim) of the warp w
+ * where 0.5 (alpha + 1) > 0.5 (alpha evaluated at the inverse network's predicted (x, y, t)), else -1.
+ * d_ws fp32, 21 P + 25 P F floats, left holding the stages (row q = p F + f; rows of fg_in / fg_out are base, x + 0.1,
+ * y + 0.05 for every point, those of inv_in / inv_out base, u + 0.1, v + 0.05 for every q):
+ *   fg_in [3P, 3] | fg_out [3P, 2] | J_fg [P, 2, 2] | delta_uv [P, 2] | inv_in [3PF, 3] | inv_out [3PF, 3] | alpha [PF] |
+ *   J_inv [PF, 2, 2] (x, y columns) | warp [PF, 2]
+ * Fails before any launch on a bad descriptor, a network of the wrong shape, P < 1, F < 1 or larger_dim < 1. */
+int vs_atlas_propagate(void* stream, const vs_imlp_desc* fg, const vs_imlp_desc* fg_inverse, const vs_imlp_desc* alpha,
+                       const float* d_points, float t_key, int P, int F, int larger_dim, float* d_ws, float* d_tracks);
+
 /* ---- measurement hooks (bench.py): per-launch CUDA-event timing on the launching stream, by kernel category
  * 0 gemm, 1 conv3x3, 2 spatial/cross attention (and the VAE's row softmax, the CLIP causal attention), 3 temporal attention, 4 groupnorm, 5 layernorm,
  * 6 other.

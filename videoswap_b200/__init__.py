@@ -1,9 +1,11 @@
 """videoswap_b200: H100-native (sm_90a) implementation of the denoising hot path of showlab/VideoSwap -- the
 `AnimateDiffUNet3DModel` forward + classifier-free guidance + DDIM step, the CLIP text encoder of the prompts, the VAE
-encode of the source frames, the VAE decode of the result and the DIFT features of tracked points -- behind the
-reference's own Python surface.
+encode of the source frames, the VAE decode of the result, the DIFT features of tracked points and the propagation of
+point drags through the layered atlas -- behind the reference's own Python surface.
 See DESIGN.md / INTEGRATION.md.  Importing this package never touches `oracle/` and there is no CPU fallback."""
 from . import formats  # noqa: F401
+from .atlas import (IMLP_Hash, atlas_dims, init_atlas_model, process_displacement_propagation,  # noqa: F401
+                    propagate_point_sequence)
 from .dift import DIFT_Demo, SDFeaturizer, extract_point_embedding  # noqa: F401
 from .pipeline import (SparsePointAdapter, TuneAVideoPipeline, TuneAVideoPipelineOutput, VideoSwapPipeline)  # noqa: F401
 from .scheduler import DDIMInverseScheduler, DDIMScheduler  # noqa: F401

@@ -35,6 +35,12 @@ _LL = C.c_longlong
 _SZ = C.c_size_t
 
 
+class ImlpDescStruct(C.Structure):
+    """vs_imlp_desc: one IMLP_Hash network (see the header)."""
+    _fields_ = [("params", _P), ("input_dim", _I), ("output_dim", _I), ("hidden_dim", _I), ("mlp_layers", _I),
+                ("pe_dim", _I), ("skip_mask", C.c_uint32), ("use_tanh", _I)]
+
+
 class GemmDescStruct(C.Structure):
     """vs_gemm_desc: one launch of the tensor-core GEMM / implicit-GEMM convolution (see the header)."""
     _fields_ = [
@@ -130,6 +136,9 @@ _SIGNATURES = {
     "vs_dift_point_sample": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
     "vs_dift_ensemble_mean": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "vs_dift_point_reduce": (_I, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "vs_imlp_forward": (_I, [_P, C.POINTER(ImlpDescStruct), _P, _I, _P]),
+    "vs_atlas_propagate": (_I, [_P, C.POINTER(ImlpDescStruct), C.POINTER(ImlpDescStruct), C.POINTER(ImlpDescStruct), _P, _F,
+                                _I, _I, _I, _P, _P]),
 }
 
 _lib = None
