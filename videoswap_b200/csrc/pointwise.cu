@@ -345,7 +345,15 @@ __global__ void __launch_bounds__(256) blend_mask_kernel(const __half* const* __
   }
 }
 
-// x_tgt = x_src + mask * (x_tgt - x_src) per (channel, frame, pixel), in fp32 (spatial_blend.py:141-142); mask [frames, hw]
+// x_tgt = x_src + mask * (x_tgt - x_src) per (channel, frame, pixel), in fp32 (spatial_blend.py:141-142); mask [frames, hw].
+// A 0 / 1 mask (all blend_mask produces) selects the source or the target bit for bit: the lerp alone would round
+// t - s and return a value near, but not equal to, the target wherever |t| << |s|.  This departs from the reference's
+// rounded lerp on purpose: at m = 1 the result is the target itself (the lerp can be a few ulps off), and the operand a
+// 0 / 1 mask does not pick is never read, so a non-finite value there (m = 0, t = inf: NaN in the lerp) does not leak
+// into the blend.  Fractional masks take the lerp unchanged.
+__device__ __forceinline__ float blend_lerp(float s, float t, float mk) {
+  return mk == 0.f ? s : (mk == 1.f ? t : s + mk * (t - s));
+}
 __global__ void latent_blend_kernel(const void* __restrict__ x_src, void* __restrict__ x_tgt, const float* __restrict__ mask,
                                     int is_f32, int channels, int frames, int hw) {
   const long long per_c = (long long)frames * hw, total = per_c * channels;
@@ -354,11 +362,11 @@ __global__ void latent_blend_kernel(const void* __restrict__ x_src, void* __rest
     if (is_f32) {
       const float s = reinterpret_cast<const float*>(x_src)[i];
       float* t = reinterpret_cast<float*>(x_tgt) + i;
-      *t = s + mk * (*t - s);
+      *t = blend_lerp(s, *t, mk);
     } else {
       const float s = __half2float(reinterpret_cast<const __half*>(x_src)[i]);
       __half* t = reinterpret_cast<__half*>(x_tgt) + i;
-      *t = __float2half_rn(s + mk * (__half2float(*t) - s));
+      *t = __float2half_rn(blend_lerp(s, __half2float(*t), mk));
     }
   }
 }
@@ -723,7 +731,10 @@ int adapter_splat(cudaStream_t st, const float* feat, const float* tracks, const
 int blend_mask(cudaStream_t st, const __half* const* maps, const int* map_res, int n_maps, int n_prompts, int frames, int heads,
                int words, const float* alpha, int pool, int h, int w, float threshold, int both, float* mask) {
   VS_REQUIRE(maps && map_res && alpha && mask && n_maps >= 1 && n_prompts >= 1 && n_prompts <= 2, "blend_mask: bad arguments");
-  VS_REQUIRE(map_res[0] * map_res[1] <= kBlendMaxRes, "blend_mask: map resolution %dx%d too large", map_res[0], map_res[1]);
+  VS_REQUIRE(frames >= 1 && heads >= 1 && words >= 1 && h >= 1 && w >= 1,
+             "blend_mask: frames %d, heads %d, words %d and target %dx%d must all be >= 1", frames, heads, words, h, w);
+  VS_REQUIRE(map_res[0] >= 1 && map_res[1] >= 1 && (long long)map_res[0] * map_res[1] <= kBlendMaxRes,
+             "blend_mask: map resolution %dx%d must be at least 1x1 and at most %d pixels", map_res[0], map_res[1], kBlendMaxRes);
   blend_mask_kernel<<<frames, 256, 0, st>>>(maps, n_maps, n_prompts, frames, heads, map_res[0], map_res[1], words, alpha, pool, h, w,
                                             threshold, both, mask);
   count_launch(1);
