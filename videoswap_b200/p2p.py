@@ -12,16 +12,16 @@ attention_store.py (`AttentionControl`, `AttentionStore`), attention_util.py (`A
     attention_store.py:95-99);
   * the blend mask and the latent blend are CUDA kernels (`vs_blend_mask`, `vs_latent_blend`).
 
-What is NOT here: the tokenizer-dependent construction of the word mappers / word selectors (seq_aligner.py, ptp_utils.py --
-pure host-side text processing on either side of this path, SURVEY 8f-4).  The edit controllers take those as tensors
-(`mapper`, `alphas`, `cross_replace_alpha`, `alpha_layers`); `from_reference()` copies them out of a controller built by the
-reference's own `make_controller`.  The reference's controller objects can also be registered unchanged (they receive device
-tensors and do their own `.cpu()`).  The small map edits (gather / lerp / einsum on [F, 8, 256, 77]) use torch ops on the
-device tensors."""
+The edit controllers take their tokenizer-dependent inputs as tensors (`mapper`, `alphas`, `cross_replace_alpha`,
+`alpha_layers`).  `make_controller` builds them from the prompts on the host (the word lookup of ptp_utils.py, the per-word
+time alphas, the refinement and replacement mappers of seq_aligner.py, restated) and moves them to the device once;
+`from_reference()` copies them out of a controller built by the reference's own `make_controller` instead.  The reference's
+controller objects can also be registered unchanged (they receive device tensors and do their own `.cpu()`).  The small map
+edits (gather / lerp / einsum on [F, 8, 256, 77]) use torch ops on the device tensors."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List, Optional, Sequence, Tuple, Union
+from typing import Dict, List, Mapping, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -368,3 +368,222 @@ def from_reference(ref_controller, additional_attention_store: AttentionStore, n
         c = AttentionReplace(ref_controller.mapper, **common)
     c.num_self_replace = tuple(ref_controller.num_self_replace)
     return c
+
+
+# ------------------------------------------------------------------------------------------------ controllers from prompts
+MAX_NUM_WORDS = 77
+
+
+def get_word_inds(text: str, word_place, tokenizer) -> List[int]:
+    """Token positions (1 = the first token after BOS) of a whitespace word of `text` (seq_aligner / ptp_utils
+    `get_word_inds`).  `word_place`: a word (every occurrence counts) or a word index.  Tokens are attributed to words by the
+    length of their decoded text, so a word the tokenizer splits yields several positions."""
+    split_text = text.split(" ")
+    if isinstance(word_place, str):
+        places = [i for i, w in enumerate(split_text) if w == word_place]
+    elif isinstance(word_place, int):
+        places = [word_place]
+    else:
+        places = list(word_place)
+    out: List[int] = []
+    if places:
+        pieces = [tokenizer.decode([t]).strip("#") for t in tokenizer.encode(text)][1:-1]
+        cur_len, ptr = 0, 0
+        for i, piece in enumerate(pieces):
+            cur_len += len(piece)
+            if ptr in places:
+                out.append(i + 1)
+            if cur_len >= len(split_text[ptr]):
+                ptr, cur_len = ptr + 1, 0
+    return out
+
+
+def _concept_word_inds(text: str, word: str, tokenizer, new_concept_cfg) -> List[int]:
+    """ptp_utils.get_word_inds: with ED-LoRA concepts the text and the word are first bound to the layer-0 concept tokens."""
+    if new_concept_cfg is not None:
+        from .formats import bind_concept_prompt
+        text, word = bind_concept_prompt(text, new_concept_cfg)[0], bind_concept_prompt(word, new_concept_cfg)[0]
+    return get_word_inds(text, word, tokenizer)
+
+
+def _window(bounds) -> Tuple[float, float]:
+    return (0.0, float(bounds)) if isinstance(bounds, (int, float)) else (bounds[0], bounds[1])
+
+
+def get_time_words_attention_alpha(prompts: Sequence[str], num_steps: int, cross_replace_steps, tokenizer,
+                                   max_num_words: int = MAX_NUM_WORDS, new_concept_cfg=None) -> torch.Tensor:
+    """ptp_utils.get_time_words_attention_alpha -> [num_steps + 1, n_prompts - 1, 1, 1, max_num_words].  Row s, word w is 1
+    while the cross-attention of w is replaced at step s.  `cross_replace_steps`: a fraction f (window [0, f)), a pair, or a
+    dict {word: fraction or pair} whose 'default_' entry (else (0, 1)) covers every word and whose other entries overwrite
+    the window of that word's tokens in each target prompt."""
+    steps = dict(cross_replace_steps) if isinstance(cross_replace_steps, Mapping) else {"default_": cross_replace_steps}
+    steps.setdefault("default_", (0.0, 1.0))
+    alpha = torch.zeros(num_steps + 1, len(prompts) - 1, max_num_words)
+
+    def update(bounds, prompt_ind, word_inds):
+        lo, hi = _window(bounds)
+        start, end = int(lo * alpha.shape[0]), int(hi * alpha.shape[0])
+        alpha[:start, prompt_ind, word_inds] = 0
+        alpha[start:end, prompt_ind, word_inds] = 1
+        alpha[end:, prompt_ind, word_inds] = 0
+
+    for i in range(len(prompts) - 1):
+        update(steps["default_"], i, torch.arange(max_num_words))
+    for key, item in steps.items():
+        if key == "default_":
+            continue
+        for i in range(1, len(prompts)):
+            inds = _concept_word_inds(prompts[i], key, tokenizer, new_concept_cfg)
+            if inds:
+                update(item, i - 1, torch.tensor(inds))
+    return alpha.reshape(num_steps + 1, len(prompts) - 1, 1, 1, max_num_words)
+
+
+def _global_align(x: Sequence[int], y: Sequence[int]) -> List[Tuple[int, int]]:
+    """Needleman-Wunsch alignment of two token sequences (match +1, mismatch -1, gap 0; ties prefer a gap in x, then a gap
+    in y, then the diagonal), traced back from the end.  Returns, for every token j of y in order, (j, i): the token of x it
+    is aligned with, or -1 for a token y inserts."""
+    nx, ny = len(x), len(y)
+    score = [[0] * (ny + 1) for _ in range(nx + 1)]
+    trace = [[0] * (ny + 1) for _ in range(nx + 1)]
+    for j in range(1, ny + 1):
+        trace[0][j] = 1
+    for i in range(1, nx + 1):
+        trace[i][0] = 2
+    trace[0][0] = 4
+    for i in range(1, nx + 1):
+        for j in range(1, ny + 1):
+            left, up = score[i][j - 1], score[i - 1][j]
+            diag = score[i - 1][j - 1] + (1 if x[i - 1] == y[j - 1] else -1)
+            best = max(left, up, diag)
+            score[i][j] = best
+            trace[i][j] = 1 if best == left else (2 if best == up else 3)
+    pairs: List[Tuple[int, int]] = []
+    i, j = nx, ny
+    while i > 0 or j > 0:
+        t = trace[i][j]
+        if t == 3:
+            i, j = i - 1, j - 1
+            pairs.append((j, i))
+        elif t == 1:
+            j -= 1
+            pairs.append((j, -1))
+        elif t == 2:
+            i -= 1
+        else:
+            break
+    pairs.reverse()
+    return pairs
+
+
+def get_refinement_mapper(prompts: Sequence[str], tokenizer, max_len: int = MAX_NUM_WORDS) -> Tuple[torch.Tensor, torch.Tensor]:
+    """seq_aligner.get_refinement_mapper -> (mapper [n - 1, max_len] int64, alphas [n - 1, max_len] float32).  Token j of
+    each target prompt reads the source token mapper[j] (-1 and alpha 0 for an inserted token); positions past the target's
+    tokens read the positions after them."""
+    x = tokenizer.encode(prompts[0])
+    mappers, alphas = [], []
+    for p in prompts[1:]:
+        y = tokenizer.encode(p)
+        base = torch.tensor(_global_align(x, y), dtype=torch.int64).reshape(-1, 2)
+        n = base.shape[0]
+        a = torch.ones(max_len)
+        a[:n] = base[:, 1].ne(-1).float()
+        m = torch.zeros(max_len, dtype=torch.int64)
+        m[:n] = base[:, 1]
+        m[n:] = len(y) + torch.arange(max_len - len(y))
+        mappers.append(m)
+        alphas.append(a)
+    return torch.stack(mappers), torch.stack(alphas)
+
+
+def get_replacement_mapper(prompts: Sequence[str], tokenizer, max_len: int = MAX_NUM_WORDS) -> torch.Tensor:
+    """seq_aligner.get_replacement_mapper -> [n - 1, max_len, max_len] float32.  The prompts must have the same number of
+    words (ValueError otherwise); each word that differs maps its source tokens onto its target tokens (1 where the counts
+    agree, else 1 / number of target tokens), every other position maps to itself."""
+    x = prompts[0]
+    words_x = x.split(" ")
+    mappers = []
+    for y in prompts[1:]:
+        words_y = y.split(" ")
+        if len(words_x) != len(words_y):
+            raise ValueError(f"attention replacement edit can only be applied on prompts with the same length but prompt A "
+                             f"has {len(words_x)} words and prompt B has {len(words_y)} words.")
+        changed = [i for i in range(len(words_y)) if words_y[i] != words_x[i]]
+        src = [get_word_inds(x, i, tokenizer) for i in changed]
+        tgt = [get_word_inds(y, i, tokenizer) for i in changed]
+        m = torch.zeros(max_len, max_len, dtype=torch.float64)
+        i = j = cur = 0
+        while i < max_len and j < max_len:
+            if cur < len(src) and src[cur][0] == i:
+                s, t = src[cur], tgt[cur]
+                if len(s) == len(t):
+                    m[s, t] = 1
+                else:
+                    for tt in t:
+                        m[s, tt] = 1 / len(t)
+                cur += 1
+                i += len(s)
+                j += len(t)
+            elif cur < len(src):
+                m[i, j] = 1
+                i, j = i + 1, j + 1
+            else:
+                m[j, j] = 1          # the reference writes the diagonal at the target position here
+                i, j = i + 1, j + 1
+        mappers.append(m.float())
+    return torch.stack(mappers)
+
+
+def word_selector(prompts: Sequence[str], words, tokenizer, new_concept_cfg=None) -> torch.Tensor:
+    """SpatialBlender's `alpha_layers` ([n_prompts, 77], 1 = a token of one of the prompt's blend words)."""
+    alpha = torch.zeros(len(prompts), MAX_NUM_WORDS)
+    for i, (prompt, words_) in enumerate(zip(prompts, words)):
+        for word in ([words_] if isinstance(words_, str) else words_):
+            ind = _concept_word_inds(prompt, word, tokenizer, new_concept_cfg)
+            if ind:
+                alpha[i, ind] = 1
+    return alpha
+
+
+def make_controller(tokenizer, prompts: List[str], is_replace_controller: bool, cross_replace_steps,
+                    self_replace_steps=0.0, blend_words=None, additional_attention_store: Optional[AttentionStore] = None,
+                    blend_th=(0.3, 0.3), NUM_DDIM_STEPS: Optional[int] = None, blend_latents: bool = False,
+                    blend_self_attention: bool = False, image_height: int = 512, image_width: int = 512, *,
+                    new_concept_cfg=None, device=None) -> AttentionControlEdit:
+    """attention_util.make_controller with the reference's signature: an AttentionReplace (equal word counts) or an
+    AttentionRefine for [source, target] prompts, with a latent SpatialBlender (prompt_choose 'both', blend window 0.2-0.8
+    of the steps) when `blend_latents` and a self-attention one ('source', 0-2) when `blend_self_attention`, both selecting
+    the tokens of `blend_words` ([source words, target words]; None or 'None': no blending).
+
+    All text work runs on the host; the tensors go to `device` once (default: CUDA when available, as the reference).
+    `new_concept_cfg` (default: the tokenizer's `new_concept_cfg` attribute, where the reference keeps it): ED-LoRA
+    concepts whose layer-0 tokens the blend words and the per-word cross_replace_steps are looked up as.  The mappers are
+    computed on the prompts as written, like the reference's.  The native controllers read the source maps and latents of
+    an inversion, so `additional_attention_store` and `NUM_DDIM_STEPS` are required."""
+    if NUM_DDIM_STEPS is None:
+        raise ValueError("make_controller needs NUM_DDIM_STEPS (the number of denoising steps)")
+    if additional_attention_store is None:
+        raise ValueError("make_controller needs additional_attention_store: the AttentionStore of the source's inversion")
+    if len(prompts) != 2:
+        raise ValueError(f"one video is edited with [source_prompt, target_prompt]; got {len(prompts)} prompts")
+    if new_concept_cfg is None:
+        new_concept_cfg = getattr(tokenizer, "new_concept_cfg", None)
+    dev = torch.device(device if device is not None else ("cuda" if torch.cuda.is_available() else "cpu"))
+    latent_blend = attention_blend = None
+    if blend_words is not None and not (isinstance(blend_words, str) and blend_words == "None"):
+        sel = word_selector(prompts, blend_words, tokenizer, new_concept_cfg).to(dev)
+        if blend_latents:
+            latent_blend = SpatialBlender(sel, start_blend=0.2, end_blend=0.8, th=blend_th, NUM_DDIM_STEPS=NUM_DDIM_STEPS,
+                                          prompt_choose="both")
+        if blend_self_attention:
+            attention_blend = SpatialBlender(sel, start_blend=0.0, end_blend=2, th=blend_th, NUM_DDIM_STEPS=NUM_DDIM_STEPS,
+                                             prompt_choose="source")
+    alpha = get_time_words_attention_alpha(prompts, NUM_DDIM_STEPS, cross_replace_steps, tokenizer,
+                                           new_concept_cfg=new_concept_cfg)
+    common = dict(num_steps=NUM_DDIM_STEPS, cross_replace_alpha=alpha.to(dev), self_replace_steps=self_replace_steps,
+                  latent_blend=latent_blend, additional_attention_store=additional_attention_store,
+                  attention_blend=attention_blend, image_height=image_height, image_width=image_width)
+    if is_replace_controller:
+        return AttentionReplace(get_replacement_mapper(prompts, tokenizer).to(dev), **common)
+    mapper, alphas = get_refinement_mapper(prompts, tokenizer)
+    return AttentionRefine(mapper.to(dev), alphas.to(dev), **common)

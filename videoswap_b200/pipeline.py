@@ -9,13 +9,14 @@ DDIM inversion (`prepare_image_latents`, `invert(video=...)`) and decodes the re
 """
 from __future__ import annotations
 
+import copy
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 from torch import nn
 
-from . import ops
+from . import formats, ops, p2p
 from .formats import bind_concept_prompt
 from .scheduler import DDIMInverseScheduler, DDIMScheduler
 from .spec import adapter_param_shapes
@@ -92,6 +93,59 @@ def _combine(eps, latents, guidance_scale, a_t, a_p, cfg):
     if not eps.is_cuda:
         raise RuntimeError("the CFG + DDIM update runs on CUDA only")
     return ops.cfg_ddim_step(eps, latents, guidance_scale, a_t, a_p, cfg=cfg)
+
+
+def edit_prompts(source_prompt: str, swap_cfg: Dict) -> Tuple[str, str, str]:
+    """The target prompt of one `editing_prompts` entry (pipeline_videoswap.py:337-346) -> (source subject, target subject,
+    target prompt).  `replace: "src -> tgt"` replaces every occurrence of src in the source prompt; `replace_other` is then
+    applied to the target prompt and must occur there."""
+    source_subject, target_subject = (s.strip() for s in swap_cfg["replace"].split("->"))
+    if source_subject not in source_prompt:
+        raise ValueError(f"replace: the source subject {source_subject!r} is not in the source prompt {source_prompt!r}")
+    target_prompt = source_prompt.replace(source_subject, target_subject)
+    if swap_cfg.get("replace_other"):
+        source_other, target_other = (s.strip() for s in swap_cfg["replace_other"].split("->"))
+        if source_other not in target_prompt:
+            raise ValueError(f"replace_other: {source_other!r} is not in the target prompt {target_prompt!r}")
+        target_prompt = target_prompt.replace(source_other, target_other)
+    return source_subject, target_subject, target_prompt
+
+
+def parse_lora_path(lora_path: str) -> Tuple[str, float, bool]:
+    """`lora_path: <file>---<alpha>` -> (file, alpha, enable_edlora); a file whose path contains 'edlora' is an ED-LoRA
+    (16 concept tokens per concept, prompts bound per cross-attention layer)."""
+    parts = lora_path.split("---")
+    if len(parts) != 2:
+        raise ValueError(f"lora_path must be '<file>---<alpha>', got {lora_path!r}")
+    return parts[0], float(parts[1]), "edlora" in parts[0]
+
+
+def select_index_list(conditions: Dict, select_point) -> Optional[List[int]]:
+    """`select_point` names -> the point columns the adapter keeps (`index_list`); None (or empty): every point."""
+    if not select_point:
+        return None
+    return [conditions["point_name2id"][name] for name in select_point]
+
+
+def draw_points(frames, conditions: Dict):
+    """The `_vispoint` frames (pipeline_videoswap.py:44-83): a green disc of radius 5 at every visible (x, y >= 0) selected
+    point, drawn IN PLACE on the given PIL frames; frames past the last tracked frame are left out of the returned list."""
+    from PIL import ImageDraw
+    tracks = conditions["pred_tracks"]
+    index_list = conditions.get("index_list")
+    out = []
+    for idx, image in enumerate(frames):
+        if idx >= len(tracks):
+            continue
+        draw = ImageDraw.Draw(image)
+        for p in range(tracks.shape[1]):
+            if index_list is not None and p not in index_list:
+                continue
+            x, y = (float(v) for v in tracks[idx][p])
+            if x >= 0 and y >= 0:
+                draw.ellipse((x - 5, y - 5, x + 5, y + 5), fill=(0, 255, 0))
+        out.append(image)
+    return out
 
 
 def _frames_to_uint8(frames) -> torch.Tensor:
@@ -235,11 +289,16 @@ class VideoSwapPipeline:
                  conditions: Optional[Dict] = None, num_inference_steps: int = 50, guidance_scale: float = 7.5,
                  t2i_guidance_scale: float = 1.0, t2i_start: float = 0.0, t2i_end: float = 1.0, controller=None,
                  output_type: str = "latent", return_dict: bool = True, callback=None, callback_steps: int = 1,
-                 max_iters: Optional[int] = None, *, prompt=None, negative_prompt=None):
+                 max_iters: Optional[int] = None, *, prompt=None, negative_prompt=None, source_prompt=None, generator=None,
+                 video_length: Optional[int] = None, num_images_per_prompt: int = 1):
         """prompt_embeds: [1,77,D] / ED-LoRA [1,16,77,D] (conditional); negative_prompt_embeds same shape (uncond).
         Or `prompt` (+ `negative_prompt`), encoded with encode_prompt (exactly one of prompt and prompt_embeds).
         latents [1,4,F,h,w] (e.g. DDIM-inverted).  Mirrors pipeline_videoswap.py:552-610: output_type "latent" returns
-        the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents)."""
+        the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents).
+        `source_prompt`, `generator` and `video_length` are accepted and unused, as in the reference's call with given
+        latents; `num_images_per_prompt` must be 1."""
+        if num_images_per_prompt != 1:
+            raise NotImplementedError("num_images_per_prompt must be 1 (one edited video per prompt)")
         if (prompt is None) == (prompt_embeds is None):
             raise ValueError("give exactly one of `prompt` and `prompt_embeds`")
         if prompt is not None and negative_prompt_embeds is not None:
@@ -362,6 +421,112 @@ class VideoSwapPipeline:
         if not return_dict:
             return latents
         return TuneAVideoInversionPipelineOutput(latents=latents.detach().clone())
+
+    @torch.no_grad()
+    def validation(self, source_video, source_conditions, source_prompt: str, editing_config: Dict,
+                   dtype=torch.float16, train_dataset=None, save_dir=None) -> Dict:
+        """The reference's `validation` (pipeline_videoswap.py:272-423), which its test.py runs on an `editing_config`:
+        invert the source video once, then run every entry of `editing_prompts` and return {key: list of PIL frames} (plus
+        `key + '_vispoint'` with `visualize_point`).
+
+          * Inversion: `invert(prompt=source_prompt, video=source_video)` over `num_inference_steps`; with `use_blend` a
+            p2p.AttentionStore (LOW_RESOURCE: no CFG) records the maps and latents and is removed afterwards.  The VAE
+            sample uses torch's default generator, as the reference's does.
+          * Per edit: `lora_path: <file>---<alpha>` is merged into the UNet and the text encoder (ED-LoRA files -- 'edlora'
+            in the path -- also add their concept tokens and bind the prompts) and restored bit-exactly after the edit; the
+            concept tokens stay in the tokenizer and the token embedding.  Conditions come from
+            `train_dataset.get_conditions(tap_path)` or a copy of `source_conditions`, with `select_point` -> index_list.
+            The target prompt is built by edit_prompts.  With `use_blend` the edit runs under p2p.make_controller's
+            AttentionRefine (latent and self-attention blending on the subject words, blend_cfg's steps and blend_th).
+            guidance_scale, t2i_guidance_scale and negative_prompt are taken from the entry first, then from the config.
+
+        Needs the pipeline's vae, text_encoder and tokenizer.  `save_dir` is only used by `visualize_attention`, which is
+        not supported (it renders with the reference's show_cross_attention)."""
+        missing = [n for n in ("vae", "text_encoder", "tokenizer") if getattr(self, n) is None]
+        if missing:
+            raise ValueError(f"validation needs a VideoSwapPipeline with {', '.join(missing)}")
+        if editing_config.get("visualize_attention", False):
+            raise NotImplementedError("visualize_attention renders maps with the reference's show_cross_attention, "
+                                      "which is not part of this package")
+        if not editing_config["use_invertion_latents"]:
+            raise ValueError("validation edits the DDIM inversion of the source video: use_invertion_latents must be true")
+        steps = editing_config["num_inference_steps"]
+        use_blend = editing_config.get("use_blend", False)
+
+        store = None
+        if use_blend:
+            store = p2p.AttentionStore()
+            store.LOW_RESOURCE = True
+            p2p.register_attention_control(self, store)
+        try:
+            inverted = self.invert(prompt=source_prompt, video=source_video, num_inference_steps=steps,
+                                   controller=store).latents.to(dtype)
+        finally:
+            if use_blend:
+                p2p.register_attention_control(self, None)
+
+        results: Dict = {}
+        for key, swap_cfg in editing_config["editing_prompts"].items():
+            unet_backup = te_backup = None
+            controller = None
+            try:
+                if swap_cfg.get("lora_path") is not None:
+                    path, alpha, enable_edlora = parse_lora_path(swap_cfg["lora_path"])
+                    lora = formats.load_edlora(path)
+                    concept_cfg = None
+                    if enable_edlora and lora["new_concept_embedding"]:
+                        concept_cfg = formats.load_new_concept(self.tokenizer, self.text_encoder,
+                                                               lora["new_concept_embedding"], enable_edlora=True)
+                    unet_backup = formats.merge_edlora_into_unet(self.unet, lora["unet"], alpha)
+                    te_backup = formats.merge_edlora_into_text_encoder(self.text_encoder, lora["text_encoder"], alpha)
+                    if enable_edlora:
+                        self.set_new_concept_cfg(concept_cfg)
+
+                if source_conditions is not None and swap_cfg.get("tap_path"):
+                    if train_dataset is None:
+                        raise ValueError(f"{key}: tap_path needs a train_dataset with get_conditions(tap_path)")
+                    conditions = train_dataset.get_conditions(swap_cfg["tap_path"])
+                else:
+                    conditions = copy.deepcopy(source_conditions)
+                if conditions is not None:
+                    conditions["index_list"] = select_index_list(conditions, swap_cfg.get("select_point"))
+
+                source_subject, target_subject, target_prompt = edit_prompts(source_prompt, swap_cfg)
+                if use_blend:
+                    width, height = source_video[0].size
+                    blend_cfg = swap_cfg.get("blend_cfg") or {}
+                    th = blend_cfg.get("blend_th", 0.3)
+                    controller = p2p.make_controller(
+                        self.tokenizer, [source_prompt, target_prompt], is_replace_controller=False,
+                        cross_replace_steps=blend_cfg.get("cross_replace_steps", 0.0),
+                        self_replace_steps=blend_cfg.get("self_replace_steps", 0.0),
+                        blend_words=[source_subject.split(" "), target_subject.split(" ")], additional_attention_store=store,
+                        blend_th=(th, th), NUM_DDIM_STEPS=steps, blend_latents=True, blend_self_attention=True,
+                        image_height=height, image_width=width, new_concept_cfg=self.new_concept_cfg,
+                        device=inverted.device)
+                    p2p.register_attention_control(self, controller)
+
+                def pick(name, default):
+                    return swap_cfg[name] if name in swap_cfg else editing_config.get(name, default)
+
+                frames = self(prompt=target_prompt, negative_prompt=pick("negative_prompt", None), conditions=conditions,
+                              latents=inverted, num_inference_steps=steps, guidance_scale=pick("guidance_scale", 7.5),
+                              t2i_guidance_scale=pick("t2i_guidance_scale", 1.0),
+                              t2i_start=editing_config.get("t2i_start", 0.0), t2i_end=editing_config.get("t2i_end", 1.0),
+                              controller=controller, output_type="pil").videos
+                results[key] = copy.deepcopy(frames)
+                if conditions is not None and editing_config.get("visualize_point", False):
+                    results[key + "_vispoint"] = draw_points(frames, conditions)
+            finally:
+                if controller is not None:
+                    p2p.register_attention_control(self, None)
+                if unet_backup is not None:
+                    formats.restore_unet(self.unet, unet_backup)
+                if te_backup is not None:
+                    formats.restore_text_encoder(self.text_encoder, te_backup)
+                if swap_cfg.get("lora_path") is not None:
+                    self.set_new_concept_cfg(None)
+        return results
 
 
 class GraphedStep:
