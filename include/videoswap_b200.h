@@ -156,6 +156,22 @@ int vs_cfg_ddim_step(void* stream, const void* d_eps2, const void* d_latents, in
 int vs_cfg_ddim_step_dev(void* stream, const void* d_eps2, const void* d_latents, int io_f32, size_t n, int cfg,
                          float guidance, const float* d_coef, void* d_out);
 
+/* The loop body's update for S videos of n_s = C F h w elements each, with diffusers 0.19.3's stochastic DDIM (eta) and
+ * the CFG rescale (pipeline_videoswap.py:578-587, rescale_noise_cfg):
+ *   eps = eps_u + g (eps_c - eps_u);  with cfg and guidance_rescale r > 0: eps *= r std(eps_c) / std(eps) + (1 - r), the
+ *   unbiased standard deviations taken per video;  x' = c_x x + c_e eps + c_n z,  c_n = eta sqrt(variance(t, t_prev)),
+ *   c_e = sqrt(1 - a_p - c_n^2) - sqrt(a_p) sqrt(1 - a_t) / sqrt(a_t),  c_x = sqrt(a_p) / sqrt(a_t).
+ * d_eps2: [2 S, n_s] (the S uncond predictions first) when cfg != 0, else [S, n_s]; d_latents, d_noise (z), d_out:
+ * [S, n_s].  d_noise may be NULL only when eta == 0.  One launch, one thread-block cluster per video; deterministic. */
+int vs_cfg_ddim_rescale_step(void* stream, const void* d_eps2, const void* d_latents, const void* d_noise, int io_f32, int S,
+                             size_t n_s, int cfg, float guidance, float alpha_t, float alpha_prev, float eta,
+                             float guidance_rescale, void* d_out);
+
+/* Same update with d_coef[0..3] = (c_x, c_e, c_n, r) in DEVICE memory (CUDA-graph replayable); d_noise NULL: no noise
+ * term. */
+int vs_cfg_ddim_rescale_step_dev(void* stream, const void* d_eps2, const void* d_latents, const void* d_noise, int io_f32,
+                                 int S, size_t n_s, int cfg, float guidance, const float* d_coef, void* d_out);
+
 /* Replaces  SparsePointAdapter.forward  (models/adapter_model.py:97-136): MLP_l(point_embedding) then bilinear splat.
  *   d_w0 [mid, E], d_b0 [mid], d_w1 [C, mid], d_b1 [C] fp16; d_point_embedding [P, E] fp32; d_tracks [F, P, 2] fp32
  *   (x, y; negative = invisible); d_point_mask [P] int32 or NULL (index_list); d_ws: >= P*(mid + C) floats scratch.

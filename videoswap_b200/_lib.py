@@ -96,6 +96,8 @@ _SIGNATURES = {
     "vs_profile_dump": (_I, [C.c_char_p]),
     "vs_cfg_ddim_step": (_I, [_P, _P, _P, _I, _SZ, _I, _F, _F, _F, _P]),
     "vs_cfg_ddim_step_dev": (_I, [_P, _P, _P, _I, _SZ, _I, _F, _P, _P]),
+    "vs_cfg_ddim_rescale_step": (_I, [_P, _P, _P, _P, _I, _I, _SZ, _I, _F, _F, _F, _F, _F, _P]),
+    "vs_cfg_ddim_rescale_step_dev": (_I, [_P, _P, _P, _P, _I, _I, _SZ, _I, _F, _P, _P]),
     "vs_adapter_level": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _F, _I, _F, _P, _P]),
     "vs_gemm_ex": (_I, [_P, C.POINTER(GemmDescStruct)]),
     "vs_pack_conv3x3": (_I, [_P, _P, _I, _I, _P]),

@@ -21,6 +21,28 @@ extern "C" int vs_cfg_ddim_step_dev(void* stream, const void* d_eps2, const void
   return cfg_ddim_step_dev((cudaStream_t)stream, d_eps2, d_latents, io_f32, n, cfg, guidance, d_coef, d_out);
 }
 
+extern "C" int vs_cfg_ddim_rescale_step(void* stream, const void* d_eps2, const void* d_latents, const void* d_noise,
+                                        int io_f32, int S, size_t n_s, int cfg, float guidance, float alpha_t,
+                                        float alpha_prev, float eta, float guidance_rescale, void* d_out) {
+  VS_REQUIRE(d_eps2 && d_latents && d_out && (d_noise || eta == 0.f), "vs_cfg_ddim_rescale_step: null pointer");
+  VS_REQUIRE(S > 0 && n_s > 0, "vs_cfg_ddim_rescale_step: S = %d and n_s = %zu must be > 0", S, n_s);
+  VS_REQUIRE(alpha_t > 0.f && alpha_t <= 1.f && alpha_prev > 0.f && alpha_prev <= 1.f,
+             "vs_cfg_ddim_rescale_step: alphas must be in (0,1]");
+  VS_REQUIRE(eta >= 0.f && (eta == 0.f || alpha_t < 1.f), "vs_cfg_ddim_rescale_step: eta must be >= 0 (and alpha_t < 1 when > 0)");
+  VS_REQUIRE(guidance_rescale >= 0.f, "vs_cfg_ddim_rescale_step: guidance_rescale must be >= 0");
+  return cfg_ddim_rescale_step((cudaStream_t)stream, d_eps2, d_latents, d_noise, io_f32, S, n_s, cfg, guidance, alpha_t,
+                               alpha_prev, eta, guidance_rescale, d_out);
+}
+
+extern "C" int vs_cfg_ddim_rescale_step_dev(void* stream, const void* d_eps2, const void* d_latents, const void* d_noise,
+                                            int io_f32, int S, size_t n_s, int cfg, float guidance, const float* d_coef,
+                                            void* d_out) {
+  VS_REQUIRE(d_eps2 && d_latents && d_out && d_coef, "vs_cfg_ddim_rescale_step_dev: null pointer");
+  VS_REQUIRE(S > 0 && n_s > 0, "vs_cfg_ddim_rescale_step_dev: S = %d and n_s = %zu must be > 0", S, n_s);
+  return cfg_ddim_rescale_step_dev((cudaStream_t)stream, d_eps2, d_latents, d_noise, io_f32, S, n_s, cfg, guidance, d_coef,
+                                   d_out);
+}
+
 extern "C" int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0, const void* d_w1, const void* d_b1, int E,
                                 int mid, int C, const float* d_pe, const float* d_tracks, const int* d_mask, int F, int P,
                                 int h, int w, float rate, int coord_fp16, float scale, float* d_ws, void* d_map) {

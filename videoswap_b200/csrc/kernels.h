@@ -165,6 +165,13 @@ int cfg_ddim_step(cudaStream_t st, const void* eps2, const void* latents, int is
 // Same, with the two DDIM coefficients (c_x, c_e) read from device memory (CUDA-graph replayable across timesteps).
 int cfg_ddim_step_dev(cudaStream_t st, const void* eps2, const void* latents, int is_f32, size_t n, int cfg,
                       float guidance, const float* d_coef, void* out);
+// S samples of n_s elements: CFG, the per-sample rescale toward std(e_c) (rescale > 0, CFG only) and the DDIM step with
+// eta: x' = c_x x + c_e e + c_n noise (noise [S, n_s] or null).  eps2: [2 S, n_s] (uncond block first) or [S, n_s].
+int cfg_ddim_rescale_step(cudaStream_t st, const void* eps2, const void* latents, const void* noise, int is_f32, int S,
+                          size_t n_s, int cfg, float guidance, float a_t, float a_prev, float eta, float rescale, void* out);
+// Same, with (c_x, c_e, c_n, rescale) read from device memory.
+int cfg_ddim_rescale_step_dev(cudaStream_t st, const void* eps2, const void* latents, const void* noise, int is_f32, int S,
+                              size_t n_s, int cfg, float guidance, const float* d_coef, void* out);
 // SparsePointAdapter splat: feat [P, C] fp32, tracks [F, P, 2] fp32 -> maps NHWC [F, h, w, C] fp16 (zeroed inside)
 int adapter_splat(cudaStream_t st, const float* feat, const float* tracks, const int* point_mask, int F, int P, int C,
                   int h, int w, float rate, int coord_fp16, float scale, __half* maps);

@@ -232,6 +232,98 @@ __global__ void cfg_ddim_kernel(const T* __restrict__ eps2, const T* __restrict_
   }
 }
 
+// ---------------------------------------------------------------------------------------------- CFG + rescale + DDIM(eta)
+// The same step for S samples of n_s elements each, with diffusers 0.19.3's stochastic DDIM (eta > 0) and the CFG
+// rescale of rescale_noise_cfg (pipeline_videoswap.py:582-584):
+//   e  = e_u + g (e_c - e_u)                                   (e = e_u without CFG)
+//   e <- e (r std(e_c) / std(e) + 1 - r)                       (CFG and r > 0 only; unbiased std over the sample)
+//   x' = c_x x + c_e e + c_n z                                 (z: the caller's noise; absent when null)
+// One thread-block cluster per sample (ncta CTAs, each a contiguous slice).  With the rescale each CTA first sums its
+// slice's shifted (sum, sum of squares) of e_c and e in fp64, the CTAs exchange the four partials through distributed
+// shared memory between two cluster barriers and add them in rank order (no atomics: bit-reproducible), and a second
+// sweep re-reads the slice (from L2) to apply the update.  The shift is the sample's first value: with fp64 partials a
+// mean of 1e3 at spread 1 keeps its variance.
+constexpr int kRsThreads = 512;
+constexpr int kRsMaxCta = 16;
+
+template <typename T>
+__global__ void __launch_bounds__(kRsThreads) cfg_ddim_rescale_kernel(
+    const T* __restrict__ eps2, const T* __restrict__ x, const T* __restrict__ z, long long ns, int S, int ncta, int cfg,
+    float g, float c_x, float c_e, float c_n, float r, const float* __restrict__ d_coef, T* __restrict__ out) {
+  __shared__ double warp_part[kRsThreads / 32][4];
+  __shared__ double part[4], tot[4];
+  if (d_coef) {   // coefficients in device memory: (c_x, c_e, c_n, r), replayable inside a CUDA graph
+    c_x = d_coef[0];
+    c_e = d_coef[1];
+    c_n = d_coef[2];
+    r = d_coef[3];
+  }
+  const int s = blockIdx.x / ncta, rank = blockIdx.x % ncta;
+  const long long chunk = (ns + ncta - 1) / ncta;
+  const long long lo = min(ns, (long long)rank * chunk), hi = min(ns, lo + chunk);
+  const T* eu = eps2 + (long long)s * ns;
+  const T* ec = eps2 + ((long long)S + s) * ns;
+  const T* xs = x + (long long)s * ns;
+  const T* zs = z ? z + (long long)s * ns : nullptr;
+  T* os = out + (long long)s * ns;
+  auto cfg_e = [&](long long i) {
+    const float u = (float)eu[i];
+    return cfg ? u + g * ((float)ec[i] - u) : u;
+  };
+  float factor = 1.f;
+  if (cfg && r > 0.f) {   // uniform over the cluster: every CTA reads the same r
+    const double kc = (double)(float)ec[0], ke = (double)cfg_e(0);
+    double sc = 0.0, qc = 0.0, se = 0.0, qe = 0.0;
+    for (long long i = lo + threadIdx.x; i < hi; i += kRsThreads) {
+      const double dc = (double)(float)ec[i] - kc, de = (double)cfg_e(i) - ke;
+      sc += dc; qc = fma(dc, dc, qc);
+      se += de; qe = fma(de, de, qe);
+    }
+    double v[4] = {sc, qc, se, qe};
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+      if (lane == 0) warp_part[wid][j] = v[j];
+    }
+    __syncthreads();
+    if (threadIdx.x < 4) {
+      double t = 0.0;
+      for (int w = 0; w < kRsThreads / 32; ++w) t += warp_part[w][threadIdx.x];   // fixed order
+      part[threadIdx.x] = t;
+    }
+    __syncthreads();
+    if (ncta > 1) cluster_sync_all();                                            // every CTA's partials are complete
+    if (threadIdx.x < 4) {
+      double t = 0.0;
+      if (ncta > 1) {
+        const uint32_t mine = smem_u32(&part[threadIdx.x]);
+        for (int c = 0; c < ncta; ++c) {                                           // rank order: deterministic
+          double pv;
+          asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(pv) : "r"(mapa_shared(mine, (uint32_t)c)));
+          t += pv;
+        }
+      } else {
+        t = part[threadIdx.x];
+      }
+      tot[threadIdx.x] = t;
+    }
+    __syncthreads();
+    const double n = (double)ns;
+    const double var_c = (tot[1] - tot[0] * tot[0] / n) / (n - 1.0);
+    const double var_e = (tot[3] - tot[2] * tot[2] / n) / (n - 1.0);
+    factor = (float)((double)r * (sqrt(var_c) / sqrt(var_e)) + (1.0 - (double)r));
+  }
+  for (long long i = lo + threadIdx.x; i < hi; i += kRsThreads) {
+    const float e = cfg_e(i) * factor;
+    float v = c_x * (float)xs[i] + c_e * e;
+    if (zs) v += c_n * (float)zs[i];
+    os[i] = (T)v;
+  }
+  if (cfg && r > 0.f && ncta > 1) cluster_sync_all();   // nobody leaves while a peer may still read its partials
+}
+
 // ---------------------------------------------------------------------------------------------- adapter splat
 __device__ __forceinline__ float r16(float v, int on) { return on ? __half2float(__float2half_rn(v)) : v; }
 
@@ -718,6 +810,60 @@ int cfg_ddim_step_dev(cudaStream_t st, const void* eps2, const void* latents, in
   count_launch(1);
   VS_CHECK_CUDA(cudaGetLastError());
   return 0;
+}
+// One launch of cfg_ddim_rescale_kernel: S clusters of ncta CTAs.  The cluster dimension is only needed when the
+// kernel may exchange statistics (CFG with a rescale factor that is > 0 or only known on the device).
+static int cfg_ddim_rescale_launch(cudaStream_t st, const void* eps2, const void* latents, const void* noise, int is_f32,
+                                   int S, size_t n_s, int cfg, float guidance, float c_x, float c_e, float c_n, float r,
+                                   const float* d_coef, void* out) {
+  const long long ns = (long long)n_s;
+  const long long want = (ns + kRsThreads * 8 - 1) / (kRsThreads * 8);      // ~8 elements per thread
+  const int ncta = want < 1 ? 1 : (want > kRsMaxCta ? kRsMaxCta : (int)want);
+  const bool cluster = cfg && (d_coef != nullptr || r > 0.f) && ncta > 1;
+  static bool configured = false;
+  if (!configured) {
+    VS_CHECK_CUDA(cudaFuncSetAttribute(cfg_ddim_rescale_kernel<float>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    VS_CHECK_CUDA(cudaFuncSetAttribute(cfg_ddim_rescale_kernel<__half>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    configured = true;
+  }
+  cudaLaunchConfig_t lc = {};
+  lc.gridDim = dim3((unsigned)(S * ncta));
+  lc.blockDim = dim3(kRsThreads);
+  lc.stream = st;
+  cudaLaunchAttribute attr[1];
+  if (cluster) {
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = ncta;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    lc.attrs = attr;
+    lc.numAttrs = 1;
+  }
+  const int esz = is_f32 ? 4 : 2;
+  // bytes: e_u (+ e_c), x, z read and x' written once; the rescale's second read of e comes from L2
+  ProfScope prof(st, PC_OTHER, (double)S * ns * esz * ((cfg ? 2 : 1) + 2 + (noise ? 1 : 0)));
+  if (is_f32)
+    VS_CHECK_CUDA(cudaLaunchKernelEx(&lc, cfg_ddim_rescale_kernel<float>, (const float*)eps2, (const float*)latents,
+                                     (const float*)noise, ns, S, ncta, cfg, guidance, c_x, c_e, c_n, r, d_coef, (float*)out));
+  else
+    VS_CHECK_CUDA(cudaLaunchKernelEx(&lc, cfg_ddim_rescale_kernel<__half>, (const __half*)eps2, (const __half*)latents,
+                                     (const __half*)noise, ns, S, ncta, cfg, guidance, c_x, c_e, c_n, r, d_coef, (__half*)out));
+  return 0;
+}
+int cfg_ddim_rescale_step(cudaStream_t st, const void* eps2, const void* latents, const void* noise, int is_f32, int S,
+                          size_t n_s, int cfg, float guidance, float a_t, float a_prev, float eta, float rescale, void* out) {
+  // diffusers 0.19.3 DDIMScheduler.step / _get_variance, in fp64 and rounded once (ops.ddim_coefficients is the same
+  // expression in Python, so host- and device-coefficient launches agree bit for bit)
+  const double at = a_t, ap = a_prev;
+  const double cn = eta == 0.f ? 0.0 : (double)eta * sqrt((1.0 - ap) / (1.0 - at) * (1.0 - at / ap));
+  const double cx = sqrt(ap) / sqrt(at);
+  const double ce = sqrt(1.0 - ap - cn * cn) - sqrt(ap) * sqrt(1.0 - at) / sqrt(at);
+  return cfg_ddim_rescale_launch(st, eps2, latents, noise, is_f32, S, n_s, cfg, guidance, (float)cx, (float)ce, (float)cn,
+                                 rescale, nullptr, out);
+}
+int cfg_ddim_rescale_step_dev(cudaStream_t st, const void* eps2, const void* latents, const void* noise, int is_f32, int S,
+                              size_t n_s, int cfg, float guidance, const float* d_coef, void* out) {
+  return cfg_ddim_rescale_launch(st, eps2, latents, noise, is_f32, S, n_s, cfg, guidance, 0.f, 0.f, 0.f, 0.f, d_coef, out);
 }
 int adapter_splat(cudaStream_t st, const float* feat, const float* tracks, const int* point_mask, int F, int P, int C,
                   int h, int w, float rate, int coord_fp16, float scale, __half* maps) {

@@ -499,12 +499,24 @@ def upsample2x(x):
     return out
 
 
-def ddim_coefficients(alpha_t: float, alpha_prev: float):
-    """(c_x, c_e) with x_prev = c_x * x + c_e * eps  (DDIM, eta = 0)."""
+def ddim_coefficients(alpha_t: float, alpha_prev: float, eta: Optional[float] = None):
+    """(c_x, c_e) with x_prev = c_x * x + c_e * eps  (DDIM, eta = 0).
+    With `eta` given: (c_x, c_e, c_n) of diffusers 0.19.3's stochastic step, x_prev = c_x x + c_e eps + c_n z, with
+    c_n = eta sqrt(variance(t, t_prev)) and c_e = sqrt(1 - a_p - c_n^2) - sqrt(a_p) sqrt(1 - a_t) / sqrt(a_t); at eta = 0
+    the first two are the values above.  The same fp64 expression as vs_cfg_ddim_rescale_step's, so device coefficients
+    rounded to fp32 reproduce the host-coefficient launch bit for bit."""
     import math
-    c_x = math.sqrt(alpha_prev) / math.sqrt(alpha_t)
-    c_e = math.sqrt(1.0 - alpha_prev) - math.sqrt(alpha_prev) * math.sqrt(1.0 - alpha_t) / math.sqrt(alpha_t)
-    return c_x, c_e
+    if eta is None:
+        c_x = math.sqrt(alpha_prev) / math.sqrt(alpha_t)
+        c_e = math.sqrt(1.0 - alpha_prev) - math.sqrt(alpha_prev) * math.sqrt(1.0 - alpha_t) / math.sqrt(alpha_t)
+        return c_x, c_e
+    if eta < 0:
+        raise ValueError(f"eta must be >= 0, got {eta}")
+    at, ap = float(alpha_t), float(alpha_prev)
+    c_n = 0.0 if eta == 0 else float(eta) * math.sqrt((1.0 - ap) / (1.0 - at) * (1.0 - at / ap))
+    c_x = math.sqrt(ap) / math.sqrt(at)
+    c_e = math.sqrt(1.0 - ap - c_n * c_n) - math.sqrt(ap) * math.sqrt(1.0 - at) / math.sqrt(at)
+    return c_x, c_e, c_n
 
 
 def cfg_ddim_step(eps2, latents, guidance, alpha_t=None, alpha_prev=None, cfg=True, out=None, coef=None):
@@ -520,6 +532,32 @@ def cfg_ddim_step(eps2, latents, guidance, alpha_t=None, alpha_prev=None, cfg=Tr
         return out
     _lib.call("vs_cfg_ddim_step", _stream(), _p(eps2), _p(latents), is_f32, latents.numel(), int(cfg), float(guidance),
               float(alpha_t), float(alpha_prev), _p(out))
+    return out
+
+
+def cfg_ddim_rescale_step(eps2, latents, guidance, alpha_t=None, alpha_prev=None, eta=0.0, guidance_rescale=0.0,
+                          noise=None, cfg=True, out=None, coef=None):
+    """The CFG combine, diffusers' rescale_noise_cfg and DDIMScheduler.step with eta for S = latents.shape[0] samples in
+    one launch (vs_cfg_ddim_rescale_step).  eps2: [2 S, ...] (uncond block first) under CFG, else [S, ...]; noise: the
+    step's standard normal draw, latents' shape and dtype (needed when eta > 0).  coef: optional device tensor [4] fp32
+    (c_x, c_e, c_n, guidance_rescale) instead of the host alphas / eta / guidance_rescale (CUDA-graph replayable)."""
+    S = latents.shape[0]
+    assert eps2.dtype == latents.dtype and eps2.is_contiguous() and latents.is_contiguous()
+    assert eps2.numel() == latents.numel() * (2 if cfg else 1), "eps2 must hold (2 if cfg else 1) x latents' elements"
+    if noise is not None:
+        assert noise.dtype == latents.dtype and noise.is_contiguous() and noise.shape == latents.shape
+    is_f32 = int(latents.dtype == torch.float32)
+    if out is None:
+        out = torch.empty_like(latents)
+    n_s = latents.numel() // S
+    if coef is not None:
+        _chk32(coef)
+        assert coef.numel() >= 4
+        _lib.call("vs_cfg_ddim_rescale_step_dev", _stream(), _p(eps2), _p(latents), _p(noise), is_f32, S, n_s, int(cfg),
+                  float(guidance), _p(coef), _p(out))
+        return out
+    _lib.call("vs_cfg_ddim_rescale_step", _stream(), _p(eps2), _p(latents), _p(noise), is_f32, S, n_s, int(cfg),
+              float(guidance), float(alpha_t), float(alpha_prev), float(eta), float(guidance_rescale), _p(out))
     return out
 
 

@@ -1,9 +1,9 @@
 """Host-side mirror of the reference's `SparsePointAdapter` (videoswap/models/adapter_model.py:50-136) and of the
 denoising part of `VideoSwapPipeline` (videoswap/pipelines/pipeline_videoswap.py:427-619 `__call__`, :622-721 `invert`).
 
-Scope (SURVEY.md 8): the loop body -- CFG batch duplication, UNet forward, CFG combine, scheduler step, adapter
-residual window -- runs on the native kernels.  The pipeline takes `prompt_embeds` and `latents` tensors and returns
-latents.  Given a `text_encoder` (videoswap_b200.text.CLIPTextModel) and the caller's `tokenizer` it also takes prompts
+Scope (SURVEY.md 8): the loop body -- CFG batch duplication, UNet forward, CFG combine (with diffusers'
+guidance_rescale), scheduler step (with DDIM eta), adapter residual window -- runs on the native kernels.  The pipeline
+takes `prompt_embeds` (one or more videos) and either `latents` or a generator to draw them from, and returns latents.  Given a `text_encoder` (videoswap_b200.text.CLIPTextModel) and the caller's `tokenizer` it also takes prompts
 (`encode_prompt`, plain or ED-LoRA); given a `vae` (videoswap_b200.vae.AutoencoderKL) it encodes the source frames for the
 DDIM inversion (`prepare_image_latents`, `invert(video=...)`) and decodes the result into frames.
 """
@@ -17,6 +17,7 @@ import torch
 from torch import nn
 
 from . import formats, ops, p2p
+from .noise import randn_tensor
 from .formats import bind_concept_prompt
 from .scheduler import DDIMInverseScheduler, DDIMScheduler
 from .spec import adapter_param_shapes
@@ -255,7 +256,8 @@ class VideoSwapPipeline:
         """The loop body on ONE video split over ranks (dist_util.ShardPlan; SURVEY 8e).  `latents` [1,4,F/k,h,w] and
         `residuals` 4 x [(F/k),C,h,w] hold THIS rank's frames; `embeds` is the full [2,...] (uncond first).  The rank runs the
         UNet on its CFG half (batch 1; GroupNorm statistics and the motion modules exchange inside the library), the two
-        halves swap their noise predictions, and both compute the same DDIM update for their frames."""
+        halves swap their noise predictions, and both compute the same DDIM update for their frames.  It takes no eta and
+        no guidance_rescale: the rescale's per-video statistics would span the frame shards."""
         from . import dist_util
         cfg = guidance_scale > 1.0
         if cfg and plan.cfg_ranks != 2:
@@ -272,16 +274,24 @@ class VideoSwapPipeline:
 
     @torch.no_grad()
     def step(self, latents: torch.Tensor, t: int, embeds: torch.Tensor, guidance_scale: float = 7.5,
-             residuals: Optional[List[torch.Tensor]] = None) -> torch.Tensor:
+             residuals: Optional[List[torch.Tensor]] = None, *, eta: float = 0.0, guidance_rescale: float = 0.0,
+             generator=None) -> torch.Tensor:
         """One loop body (pipeline_videoswap.py:556-587): CFG batch duplication -> UNet -> CFG combine -> DDIM step.
-        `embeds` is [2,...] (uncond first) when guidance_scale > 1 else [1,...]; `scheduler.set_timesteps` must have
-        been called.  Returns the new latents."""
+        `latents` is [b, 4, F, h, w]; `embeds` is [2 b,...] (the b uncond first) when guidance_scale > 1 else [b,...];
+        `scheduler.set_timesteps` must have been called.  eta > 0 adds eta sqrt(variance) times the draw
+        randn_tensor(latents.shape, generator, latents' device and dtype), as DDIMScheduler.step does; guidance_rescale > 0
+        (CFG only) rescales the guided prediction toward the conditional one's standard deviation (rescale_noise_cfg).
+        Both run in one fused kernel; without them the step is the eta = 0 kernel.  Returns the new latents."""
         cfg = guidance_scale > 1.0
         a_t, a_p = self.scheduler.alphas(t)
         x_in = torch.cat([latents] * 2) if cfg else latents
         x_in = self.scheduler.scale_model_input(x_in, t)
         eps = self.unet(x_in, t, encoder_hidden_states=embeds, down_block_additional_residuals=residuals, return_dict=False)[0]
-        return _combine(eps, latents, guidance_scale, a_t, a_p, cfg)
+        if eta == 0 and not (cfg and guidance_rescale > 0):
+            return _combine(eps, latents, guidance_scale, a_t, a_p, cfg)
+        noise = randn_tensor(latents.shape, generator, latents.device, latents.dtype) if eta > 0 else None
+        return ops.cfg_ddim_rescale_step(eps, latents, guidance_scale, a_t, a_p, eta=eta,
+                                         guidance_rescale=guidance_rescale if cfg else 0.0, noise=noise, cfg=cfg)
 
     @torch.no_grad()
     def __call__(self, prompt_embeds: Optional[torch.Tensor] = None, latents: Optional[torch.Tensor] = None,
@@ -290,28 +300,47 @@ class VideoSwapPipeline:
                  t2i_guidance_scale: float = 1.0, t2i_start: float = 0.0, t2i_end: float = 1.0, controller=None,
                  output_type: str = "latent", return_dict: bool = True, callback=None, callback_steps: int = 1,
                  max_iters: Optional[int] = None, *, prompt=None, negative_prompt=None, source_prompt=None, generator=None,
-                 video_length: Optional[int] = None, num_images_per_prompt: int = 1):
-        """prompt_embeds: [1,77,D] / ED-LoRA [1,16,77,D] (conditional); negative_prompt_embeds same shape (uncond).
-        Or `prompt` (+ `negative_prompt`), encoded with encode_prompt (exactly one of prompt and prompt_embeds).
-        latents [1,4,F,h,w] (e.g. DDIM-inverted).  Mirrors pipeline_videoswap.py:552-610: output_type "latent" returns
-        the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents).
-        `source_prompt`, `generator` and `video_length` are accepted and unused, as in the reference's call with given
-        latents; `num_images_per_prompt` must be 1."""
+                 video_length: Optional[int] = None, num_images_per_prompt: int = 1, height: Optional[int] = None,
+                 width: Optional[int] = None, eta: float = 0.0, guidance_rescale: float = 0.0):
+        """prompt_embeds: [b,77,D] / ED-LoRA [b,16,77,D] (conditional); negative_prompt_embeds same shape (uncond).
+        Or `prompt` (+ `negative_prompt`): a string, or a list of b prompts, encoded with encode_prompt (exactly one of
+        prompt and prompt_embeds).  b videos are denoised in one UNet batch; with `conditions` or a `controller` b must be 1.
+        latents [b,4,F,h,w] (e.g. DDIM-inverted), or None: prepare_latents (pipeline_videoswap.py:178-202) draws them with
+        randn_tensor(generator) at [b, 4, video_length, height / 8, width / 8] in the prompt embeddings' dtype (height and
+        width default to unet.config.sample_size * 8) and scales them by scheduler.init_noise_sigma.  `generator`: one
+        torch.Generator or a list of b.  eta > 0: DDIMScheduler.step's noise, drawn from `generator` at every step;
+        guidance_rescale > 0: rescale_noise_cfg under CFG.  Mirrors pipeline_videoswap.py:552-610: output_type "latent"
+        returns the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents).
+        `source_prompt` is accepted and unused; `num_images_per_prompt` must be 1."""
         if num_images_per_prompt != 1:
             raise NotImplementedError("num_images_per_prompt must be 1 (one edited video per prompt)")
         if (prompt is None) == (prompt_embeds is None):
             raise ValueError("give exactly one of `prompt` and `prompt_embeds`")
         if prompt is not None and negative_prompt_embeds is not None:
             raise ValueError("`prompt` takes `negative_prompt`, not `negative_prompt_embeds`")
-        if latents is None:
-            raise ValueError("VideoSwapPipeline needs `latents` (e.g. from invert)")
+        if eta < 0:
+            raise ValueError(f"eta must be >= 0, got {eta}")
+        if guidance_rescale < 0:
+            raise ValueError(f"guidance_rescale must be >= 0, got {guidance_rescale}")
+        if prompt is not None:
+            batch = 1 if isinstance(prompt, str) else len(prompt)
+        else:
+            batch = prompt_embeds.shape[0]
+        if batch > 1 and (conditions is not None or controller is not None):
+            raise ValueError("conditions and attention controllers take one video: give one prompt")
+        if isinstance(generator, (list, tuple)) and len(generator) != batch:
+            raise ValueError(f"{len(generator)} generators for a batch of {batch} videos")
+        if latents is None and video_length is None:
+            raise ValueError("drawing the latents from noise needs `video_length`")
+        if latents is not None and latents.shape[0] != batch:
+            raise ValueError(f"latents hold {latents.shape[0]} videos, the prompts {batch}")
         if output_type != "latent":
             if self.vae is None:
                 raise NotImplementedError("decoding needs a VideoSwapPipeline(..., vae=AutoencoderKL); use output_type='latent'")
             if output_type not in ("pt", "np", "pil"):
                 raise ValueError(f"output_type must be 'latent', 'pt', 'np' or 'pil', got {output_type!r}")
         cfg = guidance_scale > 1.0
-        dev = latents.device
+        dev = latents.device if latents is not None else self.device
         if prompt is not None:
             embeds = self.encode_prompt(prompt, negative_prompt, cfg)           # uncond first under CFG
         elif cfg:
@@ -322,6 +351,8 @@ class VideoSwapPipeline:
             embeds = prompt_embeds
         self.scheduler.set_timesteps(num_inference_steps)
         timesteps = self.scheduler.timesteps
+        if latents is None:
+            latents = self.prepare_latents(batch, video_length, height, width, embeds.dtype, dev, generator)
         adapter_state = None
         if conditions is not None:
             if self.adapter is None:
@@ -341,7 +372,8 @@ class VideoSwapPipeline:
             res = None
             if adapter_state is not None and len(timesteps) * t2i_start <= i <= len(timesteps) * t2i_end:
                 res = list(adapter_state)        # the UNet pops from this list (no clone needed: it never writes to them)
-            latents = self.step(latents, t, embeds, guidance_scale, res)
+            latents = self.step(latents, t, embeds, guidance_scale, res, eta=eta, guidance_rescale=guidance_rescale,
+                                generator=generator)
             if controller is not None:           # edit the latents using the attention maps (pipeline_videoswap.py:589-593)
                 latents = controller.step_callback(latents).to(latents.dtype)
             if callback is not None and i % callback_steps == 0:
@@ -354,6 +386,19 @@ class VideoSwapPipeline:
         if not return_dict:
             return video
         return TuneAVideoPipelineOutput(videos=video)
+
+    def prepare_latents(self, batch_size: int, video_length: int, height: Optional[int] = None, width: Optional[int] = None,
+                        dtype=torch.float16, device=None, generator=None) -> torch.Tensor:
+        """The initial latents of a call without given ones (pipeline_videoswap.py:178-202): randn_tensor([batch_size,
+        in_channels, video_length, height // 8, width // 8], generator) * scheduler.init_noise_sigma; height and width
+        default to unet.config.sample_size * 8."""
+        height = height or self.unet.config.sample_size * 8
+        width = width or self.unet.config.sample_size * 8
+        shape = (batch_size, self.unet.config.in_channels, video_length, height // 8, width // 8)
+        if isinstance(generator, (list, tuple)) and len(generator) != batch_size:
+            raise ValueError(f"{len(generator)} generators for a batch of {batch_size} videos")
+        latents = randn_tensor(shape, generator, device if device is not None else self.device, dtype)
+        return latents * self.scheduler.init_noise_sigma
 
     @torch.no_grad()
     def decode_latents(self, latents: torch.Tensor, output_type: str = "pil"):
@@ -533,14 +578,27 @@ class GraphedStep:
     """One loop body (CFG duplication -> UNet -> CFG combine -> DDIM update) captured once in a CUDA graph and replayed
     for every timestep: the timestep and the two DDIM coefficients live in device memory (3 floats uploaded from a
     pinned host buffer before each replay), everything else (weights, embeddings, adapter residuals, workspace) is
-    static.  Removes ~750 kernel-launch gaps per step."""
+    static.  Removes ~750 kernel-launch gaps per step.
+
+    With eta > 0 or guidance_rescale > 0 (CFG) the update is the fused rescale / stochastic-DDIM kernel and the device
+    vector also holds c_n and the rescale factor (5 floats); with eta > 0 a static noise buffer is filled eagerly from
+    the call's generator before each replay, so the graph never draws and the draws are randn_tensor's."""
 
     def __init__(self, pipe: VideoSwapPipeline, latents: torch.Tensor, embeds: torch.Tensor, guidance_scale: float = 7.5,
-                 residuals: Optional[List[torch.Tensor]] = None, inverse: bool = False, plan=None):
+                 residuals: Optional[List[torch.Tensor]] = None, inverse: bool = False, plan=None, *, eta: float = 0.0,
+                 guidance_rescale: float = 0.0):
         """inverse=True: the DDIM-inversion loop body (pipeline_videoswap.py:677-696, no CFG) -- `__call__` then takes the
-        inverse scheduler's timesteps and coefficients."""
+        inverse scheduler's timesteps and coefficients.  eta / guidance_rescale: as VideoSwapPipeline.step (not with
+        inverse=True or a frame-sharding plan)."""
         self.pipe, self.guidance, self.residuals, self.inverse = pipe, guidance_scale, residuals, inverse
         self.plan = plan if (plan is not None and plan.world > 1) else None    # sharded: latents / residuals are this rank's frames
+        if eta < 0 or guidance_rescale < 0:
+            raise ValueError("eta and guidance_rescale must be >= 0")
+        self.eta = float(eta)
+        self.rescale = float(guidance_rescale) if guidance_scale > 1.0 else 0.0     # no rescale without CFG
+        self.stochastic = self.eta > 0 or self.rescale > 0
+        if self.stochastic and (inverse or self.plan is not None):
+            raise ValueError("eta and guidance_rescale apply to the single-process denoising loop only")
         if inverse:
             assert guidance_scale <= 1.0 and residuals is None, "the inversion loop runs without CFG and without adapter residuals"
             if pipe.inverse_scheduler.num_inference_steps is None:
@@ -548,13 +606,15 @@ class GraphedStep:
         dev = latents.device
         self.lat = latents.clone().contiguous()
         self.embeds = embeds.contiguous()
-        self._h = torch.zeros(3, dtype=torch.float32).pin_memory()      # timestep, c_x, c_e
-        self._d = torch.zeros(3, dtype=torch.float32, device=dev)
+        self.noise = torch.zeros_like(self.lat) if self.eta > 0 else None
+        nd = 5 if self.stochastic else 3                                  # timestep, c_x, c_e (, c_n, rescale)
+        self._h = torch.zeros(nd, dtype=torch.float32).pin_memory()
+        self._d = torch.zeros(nd, dtype=torch.float32, device=dev)
         cur = torch.cuda.current_stream()
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):
-            self._d.copy_(torch.tensor([1.0, 1.0, 0.0]))
+            self._d.copy_(torch.tensor([1.0, 1.0, 0.0, 0.0, 0.0][:nd]))
             for _ in range(2):                                          # warm-up: workspace + weights in place
                 self._body()
         cur.wait_stream(side)
@@ -584,14 +644,24 @@ class GraphedStep:
         res = list(self.residuals) if self.residuals is not None else None
         eps = self.pipe.unet(x_in, self._d[0:1], encoder_hidden_states=self.embeds, down_block_additional_residuals=res,
                              return_dict=False)[0]
+        if self.stochastic:
+            return ops.cfg_ddim_rescale_step(eps, self.lat, self.guidance, noise=self.noise, cfg=cfg, coef=self._d[1:5])
         return ops.cfg_ddim_step(eps, self.lat, self.guidance, cfg=cfg, coef=self._d[1:3])
 
-    def __call__(self, latents: torch.Tensor, t: int) -> torch.Tensor:
-        """Runs the step at timestep t.  The returned tensor is overwritten by the next call."""
+    def __call__(self, latents: torch.Tensor, t: int, generator=None) -> torch.Tensor:
+        """Runs the step at timestep t.  The returned tensor is overwritten by the next call.  With eta > 0 the step's
+        noise is drawn from `generator` (a torch.Generator, a list of one per video, or None) before the replay."""
         a_t, a_p = (self.pipe.inverse_scheduler if self.inverse else self.pipe.scheduler).alphas(t)
-        c_x, c_e = ops.ddim_coefficients(a_t, a_p)      # the same update serves both directions: x' = c_x x + c_e eps
+        if self.stochastic:
+            c_x, c_e, c_n = ops.ddim_coefficients(a_t, a_p, self.eta)
+            vals = [float(t), c_x, c_e, c_n, self.rescale]
+            if self.noise is not None:
+                self.noise.copy_(randn_tensor(self.lat.shape, generator, self.lat.device, self.lat.dtype), non_blocking=True)
+        else:
+            c_x, c_e = ops.ddim_coefficients(a_t, a_p)      # the same update serves both directions: x' = c_x x + c_e eps
+            vals = [float(t), c_x, c_e]
         # a fresh pinned staging tensor per call: torch's caching host allocator keeps it alive until the async copy ran
-        h = torch.tensor([float(t), c_x, c_e], dtype=torch.float32).pin_memory()
+        h = torch.tensor(vals, dtype=torch.float32).pin_memory()
         self._d.copy_(h, non_blocking=True)
         if latents.data_ptr() != self.lat.data_ptr():
             self.lat.copy_(latents, non_blocking=True)

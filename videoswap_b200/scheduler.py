@@ -2,7 +2,7 @@
 fused CFG+DDIM CUDA kernel).  Semantics of diffusers 0.19.3 `DDIMScheduler` as configured by SD-1.5's
 scheduler_config.json, which is what the reference instantiates (test.py:77, pipeline_videoswap.py:503,587):
 scaled_linear betas 0.00085 -> 0.012 over 1000 train steps, 'leading' spacing, steps_offset 1, set_alpha_to_one False,
-no clipping, eta 0."""
+no clipping.  eta is the caller's (0 unless given): its noise scale eta sqrt(variance(t)) enters the fused step."""
 from __future__ import annotations
 
 from typing import List
@@ -36,6 +36,12 @@ class DDIMScheduler:
 
     def scale_model_input(self, sample, timestep=None):
         return sample
+
+    def variance(self, timestep: int) -> float:
+        """diffusers 0.19.3 `_get_variance(t, prev_t)`: (1 - a_prev) / (1 - a_t) (1 - a_t / a_prev), with
+        final_alpha_cumprod as a_prev at the last step; eta sqrt(variance) is the stochastic step's noise scale."""
+        a_t, a_p = self.alphas(timestep)
+        return (1.0 - a_p) / (1.0 - a_t) * (1.0 - a_t / a_p)
 
     def alphas(self, timestep: int):
         """(alpha_cumprod[t], alpha_cumprod[prev_t]) for the step taken at `timestep`."""

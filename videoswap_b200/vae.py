@@ -19,6 +19,7 @@ from typing import Dict, Optional
 import torch
 
 from . import ops
+from .noise import randn_tensor
 from .spec import VAEConfig, vae_encoder_param_shapes, vae_param_shapes
 from .weights import seeded_state_dict
 
@@ -136,23 +137,10 @@ class DiagonalGaussianDistribution:
         return torch.exp(self.logvar)
 
     def noise(self, generator=None) -> torch.Tensor:
-        """The standard normal draw of diffusers 0.19.3 `randn_tensor(mean.shape, generator, device, dtype=fp16)`: on the
-        generator's device when that is the CPU (then moved), one draw per frame for a list of generators."""
-        n = self.parameters.shape[0]
-        shape = (n, 4) + tuple(self.parameters.shape[2:])
-        dev = self.parameters.device
-
-        def draw(g, shp):
-            rdev = "cpu" if g is not None and g.device.type == "cpu" else dev
-            if g is not None and g.device.type != "cpu" and g.device.type != dev.type:
-                raise ValueError(f"cannot draw a {dev} tensor from a generator on {g.device}")
-            return torch.randn(shp, generator=g, device=rdev, dtype=torch.float16).to(dev)
-
-        if isinstance(generator, (list, tuple)):
-            if len(generator) != n:
-                raise ValueError(f"{len(generator)} generators for {n} frames")
-            return torch.cat([draw(g, (1,) + shape[1:]) for g in generator]).contiguous()
-        return draw(generator, shape).contiguous()
+        """The standard normal draw of diffusers 0.19.3 `randn_tensor(mean.shape, generator, device, dtype=fp16)`
+        (noise.randn_tensor): one draw per frame for a list of generators."""
+        shape = (self.parameters.shape[0], 4) + tuple(self.parameters.shape[2:])
+        return randn_tensor(shape, generator, self.parameters.device, torch.float16)
 
     def sample(self, generator=None, scale: float = 1.0, video: bool = False) -> torch.Tensor:
         """scale (mean + std noise) with the noise of `noise(generator)`, fp16 [n, 4, h, w] (video=True: [1, 4, n, h, w])."""
