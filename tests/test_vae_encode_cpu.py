@@ -55,12 +55,12 @@ def test_old_encoder_attention_names_give_the_same_weights():
 def test_decoder_only_and_partial_encoder_dicts():
     cfg = V.VAEConfig()
     dec = V.seeded_state_dict(V.vae_param_shapes(cfg), seed=7)
-    out, missing = VAE._encoder_entries(dec, cfg)
+    out, missing = VAE._convert_half(dec, V.vae_encoder_param_shapes(cfg), VAE._ENCODER_ATTN)
     assert out == {} and missing == list(V.vae_encoder_param_shapes(cfg))
     with pytest.raises(KeyError, match="missing encoder keys"):
         VAE.convert_encoder_state_dict(dec, cfg)
     partial = {**dec, "encoder.conv_in.weight": torch.zeros(128, 3, 3, 3), "quant_conv.weight": torch.zeros(8, 8, 1, 1)}
-    out, missing = VAE._encoder_entries(partial, cfg)
+    out, missing = VAE._convert_half(partial, V.vae_encoder_param_shapes(cfg), VAE._ENCODER_ATTN)
     assert set(out) == {"encoder.conv_in.weight", "quant_conv.weight"} and "encoder.conv_in.bias" in missing
     with pytest.raises(KeyError, match="encoder.conv_in.bias"):
         VAE.convert_encoder_state_dict(partial, cfg)

@@ -89,13 +89,6 @@ class SparsePointAdapter(nn.Module):
         return out
 
 
-def _combine(eps, latents, guidance_scale, a_t, a_p, cfg):
-    """CFG combine + DDIM update: the fused CUDA kernel (no CPU path)."""
-    if not eps.is_cuda:
-        raise RuntimeError("the CFG + DDIM update runs on CUDA only")
-    return ops.cfg_ddim_step(eps, latents, guidance_scale, a_t, a_p, cfg=cfg)
-
-
 def edit_prompts(source_prompt: str, swap_cfg: Dict) -> Tuple[str, str, str]:
     """The target prompt of one `editing_prompts` entry (pipeline_videoswap.py:337-346) -> (source subject, target subject,
     target prompt).  `replace: "src -> tgt"` replaces every occurrence of src in the source prompt; `replace_other` is then
@@ -288,7 +281,7 @@ class VideoSwapPipeline:
         x_in = self.scheduler.scale_model_input(x_in, t)
         eps = self.unet(x_in, t, encoder_hidden_states=embeds, down_block_additional_residuals=residuals, return_dict=False)[0]
         if eta == 0 and not (cfg and guidance_rescale > 0):
-            return _combine(eps, latents, guidance_scale, a_t, a_p, cfg)
+            return ops.cfg_ddim_step(eps, latents, guidance_scale, a_t, a_p, cfg=cfg)
         noise = randn_tensor(latents.shape, generator, latents.device, latents.dtype) if eta > 0 else None
         return ops.cfg_ddim_rescale_step(eps, latents, guidance_scale, a_t, a_p, eta=eta,
                                          guidance_rescale=guidance_rescale if cfg else 0.0, noise=noise, cfg=cfg)

@@ -9,17 +9,15 @@ for 12 layers): clip_embed, then per pre-LN block  LN1 -> one QKV GEMM on a pack
 final LayerNorm.  The tokenizer is the caller's (transformers' CLIPTokenizer from the checkpoint's tokenizer/ folder)."""
 from __future__ import annotations
 
-import json
-import os
 from collections import OrderedDict, namedtuple
-from dataclasses import dataclass, fields
+from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
 
 import torch
 
 from . import ops
 from .spec import CLIPTextConfig, clip_text_param_shapes
-from .weights import seeded_state_dict
+from .weights import config_kwargs, missing_keys_text, read_pretrained_dir, seeded_state_dict
 
 TOKEN_EMBEDDING = "text_model.embeddings.token_embedding.weight"
 POSITION_EMBEDDING = "text_model.embeddings.position_embedding.weight"
@@ -90,28 +88,13 @@ class CLIPTextModel:
     def from_config(cls, config, **kw):
         """transformers-style: the keys of CLIPTextConfig are used, the rest of a config.json ignored; a config other than
         SD-1.5's raises (check_config)."""
-        if not isinstance(config, dict):
-            config = config.to_dict()
-        known = {f.name for f in fields(CLIPTextConfig)}
-        return cls(**kw, **{k: v for k, v in config.items() if k in known})
+        return cls(**kw, **config_kwargs(config, CLIPTextConfig))
 
     @classmethod
     def from_pretrained(cls, path: str, subfolder: Optional[str] = "text_encoder", device="cuda"):
         """A local diffusers / transformers directory: config.json + model.safetensors (or pytorch_model.bin)."""
-        d = os.path.join(path, subfolder) if subfolder else path
-        cfg_path = os.path.join(d, "config.json")
-        if not os.path.exists(cfg_path):
-            raise RuntimeError(f"{cfg_path} not found")
-        with open(cfg_path) as f:
-            m = cls.from_config(json.load(f), init="empty", device=device)
-        st, bn = os.path.join(d, "model.safetensors"), os.path.join(d, "pytorch_model.bin")
-        if os.path.exists(st):
-            from safetensors.torch import load_file
-            sd = load_file(st)
-        elif os.path.exists(bn):
-            sd = torch.load(bn, map_location="cpu", weights_only=True)
-        else:
-            raise RuntimeError(f"no model.safetensors / pytorch_model.bin in {d}")
+        config, sd = read_pretrained_dir(path, subfolder, "model.safetensors", "pytorch_model.bin")
+        m = cls.from_config(config, init="empty", device=device)
         m.load_state_dict(sd)
         return m
 
@@ -137,8 +120,7 @@ class CLIPTextModel:
             staged[k] = v
         missing = [k for k in shapes if k not in staged]
         if strict and missing:
-            raise KeyError(f"missing keys in the CLIP text encoder state_dict: {missing[:5]}"
-                           f"{' ...' if len(missing) > 5 else ''} ({len(missing)} keys)")
+            raise KeyError(f"missing keys in the CLIP text encoder state_dict: {missing_keys_text(missing)}")
         for k, v in staged.items():
             cur = self._params.get(k)
             if cur is not None and cur.shape == v.shape:

@@ -430,6 +430,27 @@ class AnimateDiffUNet3DModel(nn.Module):
             torch.cuda.current_stream().synchronize()   # staging tensors die at the end of the iteration
         self._dirty = False
 
+    def _prepare_inputs(self, dev, timestep, n, encoder_hidden_states=None, sample_dtype=None):
+        """What every CUDA entry point does before its launch.  It refuses a device other than CUDA and a sample dtype
+        other than fp16 / fp32 (sample_dtype None: there is no sample) before any weight upload, then syncs the weights.
+        Returns (t, ehs): the timestep (a number, or a tensor of 1 or n values) as a contiguous fp32 [n] tensor on dev,
+        and encoder_hidden_states as a contiguous fp16 tensor on dev (None when not given)."""
+        if dev.type != "cuda":
+            raise RuntimeError("AnimateDiffUNet3DModel (videoswap_b200) runs on CUDA only: there is no CPU path")
+        if sample_dtype is not None and sample_dtype not in (torch.float16, torch.float32):
+            raise TypeError("sample must be fp16 or fp32")
+        with torch.cuda.device(dev):
+            self._sync_weights(dev)
+            if torch.is_tensor(timestep):
+                t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
+            else:
+                t = torch.tensor([float(timestep)], dtype=torch.float32, device=dev)
+            t = t.expand(n).contiguous()
+            ehs = None
+            if encoder_hidden_states is not None:
+                ehs = encoder_hidden_states.to(device=dev, dtype=torch.float16).contiguous()
+        return t, ehs
+
     def _check_processors(self):
         """Validates the processors the reference's helpers may have swapped in and returns the attention controller the
         control processors carry (utils/p2p_utils/attention_register.py), or None."""
@@ -483,8 +504,6 @@ class AnimateDiffUNet3DModel(nn.Module):
                 class_labels=None, attention_mask=None, cross_attention_kwargs=None,
                 down_block_additional_residuals: Optional[List[torch.Tensor]] = None, return_dict: bool = True,
                 _taps: Optional[dict] = None):
-        if not sample.is_cuda:
-            raise RuntimeError("AnimateDiffUNet3DModel (videoswap_b200) runs on CUDA only: there is no CPU path")
         if class_labels is not None or attention_mask is not None:
             raise NotImplementedError("class_labels / attention_mask are unused on the reference's path and unsupported")
         if sample.dim() != 5:
@@ -499,18 +518,10 @@ class AnimateDiffUNet3DModel(nn.Module):
                                       "rebuilds each map's height and width from its token count and the aspect ratio)")
         if down_block_additional_residuals is not None:
             self._check_residuals(down_block_additional_residuals, B * F, H, W)
+        t, ehs = self._prepare_inputs(dev, timestep, B, encoder_hidden_states, sample.dtype)
         with torch.cuda.device(dev):
-            self._sync_weights(dev)
             io_f32 = sample.dtype == torch.float32
-            if sample.dtype not in (torch.float16, torch.float32):
-                raise TypeError("sample must be fp16 or fp32")
             x = sample.contiguous()
-            if torch.is_tensor(timestep):
-                t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
-            else:
-                t = torch.tensor([float(timestep)], dtype=torch.float32, device=dev)
-            t = t.expand(B).contiguous()
-            ehs = encoder_hidden_states.to(device=dev, dtype=torch.float16).contiguous()
             if ehs.dim() == 4:
                 layers, tokens = ehs.shape[1], ehs.shape[2]
             elif ehs.dim() == 3:
@@ -583,12 +594,8 @@ class AnimateDiffUNet3DModel(nn.Module):
         module skipped -- up to and including up block `up_ft_index` with its up-sampler.  sample [N, C, 1, H, W] (fp16 /
         fp32; every image on the batch axis, so each one gets its own GroupNorm statistics), encoder_hidden_states
         [N, 77, D] -> up_ft[up_ft_index] as NHWC fp16 [N, h_k, w_k, C_k]."""
-        if not sample.is_cuda:
-            raise RuntimeError("AnimateDiffUNet3DModel (videoswap_b200) runs on CUDA only: there is no CPU path")
         if sample.dim() != 5 or sample.shape[2] != 1 or sample.shape[1] != self.cfg.in_channels:
             raise ValueError(f"expected sample [N, {self.cfg.in_channels}, 1, H, W], got {tuple(sample.shape)}")
-        if sample.dtype not in (torch.float16, torch.float32):
-            raise TypeError("sample must be fp16 or fp32")
         if not 0 <= int(up_ft_index) <= 3:
             raise ValueError(f"up_ft_index must be in 0..3, got {up_ft_index}")
         N, _, _, H, W = sample.shape
@@ -600,15 +607,9 @@ class AnimateDiffUNet3DModel(nn.Module):
         k = int(up_ft_index)
         lh, lw = self.level_sizes(H, W)[2 - k] if k < 3 else (H, W)
         ck = self.cfg.block_out_channels[3 - k]
+        t, ehs = self._prepare_inputs(dev, timestep, N, encoder_hidden_states, sample.dtype)
         with torch.cuda.device(dev):
-            self._sync_weights(dev)
             x = sample.contiguous()
-            if torch.is_tensor(timestep):
-                t = timestep.to(device=dev, dtype=torch.float32).reshape(-1)
-            else:
-                t = torch.tensor([float(timestep)], dtype=torch.float32, device=dev)
-            t = t.expand(N).contiguous()
-            ehs = encoder_hidden_states.to(device=dev, dtype=torch.float16).contiguous()
             out = torch.empty((N, lh, lw, ck), dtype=torch.float16, device=dev)
             _lib.call("vs_unet_forward_features", self._handle, torch.cuda.current_stream().cuda_stream, x.data_ptr(),
                       int(x.dtype == torch.float32), N, 1, H, W, t.data_ptr(), ehs.data_ptr(), ehs.shape[1], 0, k,
@@ -621,13 +622,10 @@ class AnimateDiffUNet3DModel(nn.Module):
         """The forward's time embedding for timesteps [B] -> (emb fp32 [B, time_embed_dim], proj fp32 [B, tproj_n]): proj
         holds every resnet's time_emb_proj(SiLU(emb)) side by side, in the order the library registers the resnets."""
         dev = self.conv_in.weight.device
-        if dev.type != "cuda":
-            raise RuntimeError("AnimateDiffUNet3DModel (videoswap_b200) runs on CUDA only: there is no CPU path")
+        B = timesteps.numel()
+        t, _ = self._prepare_inputs(dev, timesteps, B)
         tproj_n = sum(m.time_emb_proj.weight.shape[0] for m in self.modules() if isinstance(getattr(m, "time_emb_proj", None), _Holder))
         with torch.cuda.device(dev):
-            self._sync_weights(dev)
-            t = timesteps.to(device=dev, dtype=torch.float32).reshape(-1).contiguous()
-            B = t.numel()
             emb = torch.empty((B, self.cfg.time_embed_dim), dtype=torch.float32, device=dev)
             proj = torch.empty((B, tproj_n), dtype=torch.float32, device=dev)
             _lib.call("vs_unet_time_embedding", self._handle, torch.cuda.current_stream().cuda_stream, t.data_ptr(), B,

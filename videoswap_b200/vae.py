@@ -10,10 +10,8 @@ softmax: S = Q K^T into one [hw, hw_pad] buffer, P = softmax(S / sqrt(512)) in p
 encoder's stride-2 down-samplers run as implicit GEMMs on parity views of their input (ops.downsample_conv3x3)."""
 from __future__ import annotations
 
-import json
 import math
-import os
-from dataclasses import dataclass, fields
+from dataclasses import dataclass
 from typing import Dict, Optional
 
 import torch
@@ -21,14 +19,16 @@ import torch
 from . import ops
 from .noise import randn_tensor
 from .spec import VAEConfig, vae_encoder_param_shapes, vae_param_shapes
-from .weights import seeded_state_dict
+from .weights import config_kwargs, missing_keys_text, read_pretrained_dir, seeded_state_dict
 
 EPS = 1e-6                     # resnet_eps of the SD-1.5 decoder (GroupNorms of resnets, attention and conv_norm_out)
 CONV_OUT_PAD = 8               # conv_out's 3 output channels padded to 8 so the conv kernel's stores stay 16-byte aligned
 
 # Pre-0.14 diffusers names of the mid-block attention, still shipped in SD-1.5 VAE files ([C, C] or 1x1-conv [C, C, 1, 1])
 _OLD_ATTN = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
-_IGNORED_PREFIXES = ("encoder.", "quant_conv.")   # the encode half: accepted so that a whole VAE file loads
+_ENCODER_PREFIXES = ("encoder.", "quant_conv.")   # the encode half's keys; every other key belongs to the decode half
+_DECODER_ATTN = "decoder.mid_block.attentions.0"
+_ENCODER_ATTN = "encoder.mid_block.attentions.0"
 
 
 @dataclass
@@ -36,19 +36,20 @@ class DecoderOutput:
     sample: torch.Tensor
 
 
-def convert_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str, torch.Tensor]:
-    """A full or decoder-only AutoencoderKL state_dict -> the decoder keys of vae_param_shapes(cfg), in their shapes.
-    Old attention names are renamed, encoder / quant_conv keys dropped; any other unknown key, a wrong shape or a missing
-    decoder key raises."""
-    shapes = vae_param_shapes(cfg)
+def _convert_half(sd: Dict[str, torch.Tensor], shapes, attn: str):
+    """The keys of one VAE half in sd, renamed and reshaped to that half's `shapes` -> (dict, missing keys).  attn is the
+    half's mid-block attention: under "encoder." the half is the encoder / quant_conv keys, otherwise every other key;
+    keys of the other half are skipped.  Old attention names under attn are renamed; a key of the half that `shapes`
+    does not know, a key given twice or a wrong shape raises."""
+    encoder = attn.startswith("encoder.")
     out = {}
     for k, v in sd.items():
-        if k.startswith(_IGNORED_PREFIXES):
+        if k.startswith(_ENCODER_PREFIXES) != encoder:
             continue
         name = k
         head, _, leaf = k.rpartition(".")
-        attn, _, old = head.rpartition(".")
-        if attn == "decoder.mid_block.attentions.0" and old in _OLD_ATTN:
+        parent, _, old = head.rpartition(".")
+        if parent == attn and old in _OLD_ATTN:
             name = f"{attn}.{_OLD_ATTN[old]}.{leaf}"
         if name not in shapes:
             raise KeyError(f"unexpected key in the VAE state_dict: {k}")
@@ -56,36 +57,7 @@ def convert_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str,
             raise KeyError(f"{k}: {name} is given twice (old and new attention names)")
         want = shapes[name]
         if tuple(v.shape) != want:
-            if name.startswith(attn + ".") and len(want) == 2 and tuple(v.shape) == want + (1, 1):
-                v = v.reshape(want)
-            else:
-                raise ValueError(f"{k}: shape {tuple(v.shape)}, expected {want}")
-        out[name] = v
-    missing = [k for k in shapes if k not in out]
-    if missing:
-        raise KeyError(f"missing decoder keys in the VAE state_dict: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
-    return out
-
-
-def _encoder_entries(sd: Dict[str, torch.Tensor], cfg: VAEConfig):
-    """The encoder / quant_conv keys of sd renamed and reshaped to vae_encoder_param_shapes(cfg) -> (dict, missing keys).
-    Decoder keys are skipped; an unknown encoder key, a key given twice or a wrong shape raises."""
-    shapes = vae_encoder_param_shapes(cfg)
-    out = {}
-    for k, v in sd.items():
-        if not k.startswith(_IGNORED_PREFIXES):
-            continue
-        name = k
-        head, _, leaf = k.rpartition(".")
-        attn, _, old = head.rpartition(".")
-        if attn == "encoder.mid_block.attentions.0" and old in _OLD_ATTN:
-            name = f"{attn}.{_OLD_ATTN[old]}.{leaf}"
-        if name not in shapes:
-            raise KeyError(f"unexpected key in the VAE state_dict: {k}")
-        if name in out:
-            raise KeyError(f"{k}: {name} is given twice (old and new attention names)")
-        want = shapes[name]
-        if tuple(v.shape) != want:
+            # the attention's linear weights, the only 2-D entries, may come as 1x1-conv weights
             if name.startswith(attn + ".") and len(want) == 2 and tuple(v.shape) == want + (1, 1):
                 v = v.reshape(want)
             else:
@@ -94,17 +66,23 @@ def _encoder_entries(sd: Dict[str, torch.Tensor], cfg: VAEConfig):
     return out, [k for k in shapes if k not in out]
 
 
-def _missing_text(missing) -> str:
-    return f"{missing[:5]}{' ...' if len(missing) > 5 else ''} ({len(missing)} keys)"
+def convert_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str, torch.Tensor]:
+    """A full or decoder-only AutoencoderKL state_dict -> the decoder keys of vae_param_shapes(cfg), in their shapes.
+    Old attention names are renamed, encoder / quant_conv keys dropped; any other unknown key, a wrong shape or a missing
+    decoder key raises."""
+    out, missing = _convert_half(sd, vae_param_shapes(cfg), _DECODER_ATTN)
+    if missing:
+        raise KeyError(f"missing decoder keys in the VAE state_dict: {missing_keys_text(missing)}")
+    return out
 
 
 def convert_encoder_state_dict(sd: Dict[str, torch.Tensor], cfg: VAEConfig) -> Dict[str, torch.Tensor]:
     """A full AutoencoderKL state_dict -> the encoder / quant_conv keys of vae_encoder_param_shapes(cfg), in their shapes.
     The same old attention names as convert_state_dict are renamed (encoder.mid_block.attentions.0); decoder keys are
     skipped; an unknown encoder key, a wrong shape or a missing encoder key raises."""
-    out, missing = _encoder_entries(sd, cfg)
+    out, missing = _convert_half(sd, vae_encoder_param_shapes(cfg), _ENCODER_ATTN)
     if missing:
-        raise KeyError(f"missing encoder keys in the VAE state_dict: {_missing_text(missing)}")
+        raise KeyError(f"missing encoder keys in the VAE state_dict: {missing_keys_text(missing)}")
     return out
 
 
@@ -165,6 +143,12 @@ def attend(q, k, v, s, vt, out):
     return ops.gemm(s, vt, out=out)
 
 
+def _tap(taps, name, t):
+    """Records a block's NHWC output in the executors' debugging dict, when one is given."""
+    if taps is not None:
+        taps[name] = t
+
+
 class AutoencoderKL:
     """diffusers' AutoencoderKL (decode and encode) on CUDA.  init="seeded" draws test weights for both halves
     (weights.seeded_state_dict), "empty" waits for load_state_dict."""
@@ -191,28 +175,14 @@ class AutoencoderKL:
             config = config.to_dict()
         if config.get("act_fn", "silu") != "silu":
             raise ValueError(f"unsupported act_fn {config['act_fn']!r}")
-        known = {f.name for f in fields(VAEConfig)}
-        return cls(**kw, **{k: (tuple(v) if isinstance(v, list) else v) for k, v in config.items() if k in known})
+        return cls(**kw, **config_kwargs(config, VAEConfig))
 
     @classmethod
     def from_pretrained(cls, path: str, subfolder: Optional[str] = "vae", device="cuda"):
         """A local diffusers directory: config.json + diffusion_pytorch_model.safetensors (or .bin)."""
-        d = os.path.join(path, subfolder) if subfolder else path
-        cfg_path = os.path.join(d, "config.json")
-        if not os.path.exists(cfg_path):
-            raise RuntimeError(f"{cfg_path} not found")
-        with open(cfg_path) as f:
-            m = cls.from_config(json.load(f), init="empty", device=device)
-        st, bn = os.path.join(d, "diffusion_pytorch_model.safetensors"), os.path.join(d, "diffusion_pytorch_model.bin")
-        if os.path.exists(st):
-            from safetensors.torch import load_file
-            sd = load_file(st)
-        elif os.path.exists(bn):
-            sd = torch.load(bn, map_location="cpu", weights_only=True)
-        else:
-            raise RuntimeError(f"no diffusion_pytorch_model.safetensors / .bin in {d}")
-        m.load_state_dict(sd)
-        return m
+        config, sd = read_pretrained_dir(path, subfolder, "diffusion_pytorch_model.safetensors",
+                                         "diffusion_pytorch_model.bin")
+        return cls.from_config(config, init="empty", device=device).load_state_dict(sd)
 
     # ------------------------------------------------------------------------------------------------ weights
     def load_state_dict(self, sd: Dict[str, torch.Tensor]):
@@ -222,7 +192,7 @@ class AutoencoderKL:
         missing keys."""
         if self.device.type != "cuda":
             raise RuntimeError("AutoencoderKL (videoswap_b200) runs on CUDA only")
-        enc, self._enc_missing = _encoder_entries(sd, self.config)
+        enc, self._enc_missing = _convert_half(sd, vae_encoder_param_shapes(self.config), _ENCODER_ATTN)
         sd = convert_state_dict(sd, self.config)
         self._w = self._pack_decoder(sd)
         self._we = self._pack_encoder(enc) if not self._enc_missing else None
@@ -334,6 +304,22 @@ class AutoencoderKL:
         wo, bo = a["out"]
         return ops.gemm(o, wo, bias=bo, residual=x.view(n * hw, C)).view(n, H, W, C)
 
+    def _mid_block(self, x, w, taps):
+        """UNetMidBlock2D of either half: resnet, attention, resnet."""
+        x = self._resnet(x, w["mid"][0])
+        x = self._attention(x, w["attn"])
+        _tap(taps, "mid_block.attentions.0", x)
+        x = self._resnet(x, w["mid"][1])
+        _tap(taps, "mid_block", x)
+        return x
+
+    def _out(self, x, w, taps):
+        """The tail of either half: conv_out(silu(conv_norm_out(x)))."""
+        x = ops.groupnorm(x, *w["norm_out"], self._groups(), EPS, silu=True)
+        x = ops.conv3x3(x, *w["conv_out"])
+        _tap(taps, "conv_out", x)
+        return x
+
     def _run(self, z, divisor, fmt, taps=None):
         """post_quant_conv(z / divisor) -> Decoder -> image_postprocess(fmt).  taps: dict that receives each block's NHWC
         output (debugging)."""
@@ -344,30 +330,18 @@ class AutoencoderKL:
         if z.dim() != 4 or z.shape[1] != self.config.latent_channels:
             raise ValueError(f"expected latents [n, {self.config.latent_channels}, h, w], got {tuple(z.shape)}")
         w = self._w
-
-        def tap(name, t):
-            if taps is not None:
-                taps[name] = t
-
         z = z.contiguous() if z.dtype in (torch.float16, torch.float32) else z.float().contiguous()
         x = ops.vae_latent_in(z, divisor, w["latent_in"])
         x = ops.conv_in(x, *w["conv_in"])
-        tap("conv_in", x)
-        x = self._resnet(x, w["mid"][0])
-        x = self._attention(x, w["attn"])
-        tap("mid_block.attentions.0", x)
-        x = self._resnet(x, w["mid"][1])
-        tap("mid_block", x)
+        _tap(taps, "conv_in", x)
+        x = self._mid_block(x, w, taps)
         for i, blk in enumerate(w["up"]):
             for r in blk["resnets"]:
                 x = self._resnet(x, r)
             if blk["upsampler"] is not None:
                 x = ops.upsample_conv3x3_packed(x, *blk["upsampler"])
-            tap(f"up_blocks.{i}", x)
-        x = ops.groupnorm(x, *w["norm_out"], self._groups(), EPS, silu=True)
-        x = ops.conv3x3(x, *w["conv_out"])
-        tap("conv_out", x)
-        return ops.image_postprocess(x, fmt)
+            _tap(taps, f"up_blocks.{i}", x)
+        return ops.image_postprocess(self._out(x, w, taps), fmt)
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):
@@ -397,7 +371,7 @@ class AutoencoderKL:
         (CUDA) -> the moments fp16 [n, 8, H / 8, W / 8].  taps: dict that receives each block's NHWC output (debugging)."""
         if self._we is None:
             raise RuntimeError("AutoencoderKL has no encoder weights: the last state_dict lacked "
-                               + _missing_text(self._enc_missing))
+                               + missing_keys_text(self._enc_missing))
         if not x.is_cuda:
             raise RuntimeError("AutoencoderKL (videoswap_b200) runs on CUDA only")
         if x.dim() != 4:
@@ -406,29 +380,17 @@ class AutoencoderKL:
         if H % 8 or W % 8:
             raise ValueError(f"the encoder takes images whose height and width are multiples of 8, got {tuple(x.shape)}")
         w = self._we
-
-        def tap(name, t):
-            if taps is not None:
-                taps[name] = t
-
         x = ops.vae_image_in(x.contiguous())
         x = ops.conv_in(x, *w["conv_in"])
-        tap("conv_in", x)
+        _tap(taps, "conv_in", x)
         for i, blk in enumerate(w["down"]):
             for r in blk["resnets"]:
                 x = self._resnet(x, r)
             if blk["downsampler"] is not None:
                 x = ops.downsample_conv3x3(x, *blk["downsampler"])
-            tap(f"down_blocks.{i}", x)
-        x = self._resnet(x, w["mid"][0])
-        x = self._attention(x, w["attn"])
-        tap("mid_block.attentions.0", x)
-        x = self._resnet(x, w["mid"][1])
-        tap("mid_block", x)
-        x = ops.groupnorm(x, *w["norm_out"], self._groups(), EPS, silu=True)
-        x = ops.conv3x3(x, *w["conv_out"])
-        tap("conv_out", x)
-        return ops.vae_moments(x, w["moments"])
+            _tap(taps, f"down_blocks.{i}", x)
+        x = self._mid_block(x, w, taps)
+        return ops.vae_moments(self._out(x, w, taps), w["moments"])
 
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True):
