@@ -190,7 +190,8 @@ int vs_adapter_level(void* stream, const void* d_w0, const void* d_b0, const voi
  *   an odd output axis, which has 3 taps along it (6 or 9 in all; see vs_upsample_conv3x3_sized for the panels).
  *   Epilogue: + bias[n] + rowvec[((pix / pix_per_batch) % rv_mod if rv_mod > 0), n] (row stride ldrv, 0 = N) + residual[pix, n]
  *   (row stride ldr; may alias `out`); mode 1 = GEGLU on packed weights (N / 2 output columns); mode 2 = quick-GELU,
- *   fp16(v sigmoid(1.702 v)) with v = acc + bias in fp32 (CLIP's MLP fc1: taps 1, bias only, N % 32 == 0, BLOCK_N 128 / 256).  Folded LayerNorm of A:
+ *   fp16(v sigmoid(1.702 v)) with v = acc + bias in fp32 (CLIP's MLP fc1: taps 1, bias only, N % 32 == 0, BLOCK_N 128 / 256);
+ *   mode 3 = ReLU, fp16(max(acc + bias, 0)) (the T2I-Adapter's block1: taps 9, one source, bias only, N % 32 == 0).  Folded LayerNorm of A:
  *   ln_u [N] with ln_stats [M, 2] (rstd, -mean rstd) or ln_parts [ln_nparts][M][2] (sum, sum of squares).
  *   ln_sums_out [n_tiles][M][2]: (sum, sum of squares) of the stored fp16 outputs per row and column tile of width BN.
  *   force_bn 0 = automatic column-tile width, else 64 / 128 / 160 / 256.
@@ -319,6 +320,20 @@ int vs_vae_moments(void* stream, const void* d_x, int nimg, int h, int w, const 
  * [1, 4, nimg, h, w] (layout 1: the frames of one video, as the inversion loop takes them). */
 int vs_vae_posterior(void* stream, const void* d_params, const void* d_noise, int nimg, int h, int w, float scale, int layout,
                      void* d_out);
+
+/* ---- T2I-Adapter (diffusers 0.19.3 T2IAdapter with adapter_type "full_adapter": the reference's image-condition branch,
+ * pipeline_videoswap.py:538-546).  The adapter is a sequence of vs_gemm_ex (conv_in and block1 as taps 9, block1 with
+ * mode 3; in_conv and block2 as taps 1, block2 with the residual) and these three. */
+/* Entry: uint8 frames d_x [nimg, H, W, channels] (channels 1 = "L" or 3 = "RGB", H and W multiples of 8, 8-byte aligned) ->
+ * the PixelUnshuffle(8) of fp16(fp32(u) / 255) as NHWC fp16 d_out [nimg, H / 8, W / 8, 64 channels], channel
+ * c 64 + 8 i + j of output pixel (y, x) = input pixel (8 y + i, 8 x + j), channel c (torch's PixelUnshuffle order). */
+int vs_t2i_image_in(void* stream, const void* d_x, int nimg, int H, int W, int channels, void* d_out);
+/* AvgPool2d(2, stride 2) of NHWC fp16 d_x [nimg, H, W, C] (H, W even, C % 8 == 0) -> d_out [nimg, H / 2, W / 2, C]:
+ * the four values summed in fp32, times 0.25, rounded once. */
+int vs_avgpool2x2(void* stream, const void* d_x, int nimg, int H, int W, int C, void* d_out);
+/* d_out[i] = fp16(fp32(d_x[i]) * scale) for n fp16 values (n % 8 == 0, 16-byte aligned; d_out may be d_x): the
+ * t2i_guidance_scale multiply of the adapter's fp16 features, rounded as torch rounds `v * scale`. */
+int vs_scale_f16(void* stream, const void* d_x, size_t n, float scale, void* d_out);
 
 /* ---- CLIP text encoder (transformers CLIPTextModel, SD-1.5's text_encoder; the reference's prompt encoding,
  * pipeline_videoswap.py:273-423 and utils/edlora_util.py:116-196).  The encoder is a sequence of vs_layernorm, vs_gemm_ex

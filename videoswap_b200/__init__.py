@@ -11,6 +11,7 @@ from .pipeline import (SparsePointAdapter, TuneAVideoPipeline, TuneAVideoPipelin
 from .scheduler import DDIMInverseScheduler, DDIMScheduler  # noqa: F401
 from .spec import (CLIPTextConfig, UNetConfig, VAEConfig, adapter_param_shapes, clip_text_param_shapes,  # noqa: F401
                    unet_param_shapes, vae_encoder_param_shapes, vae_param_shapes)
+from .t2i_adapter import T2IAdapter, T2IAdapterConfig, t2i_adapter_param_shapes  # noqa: F401
 from .text import CLIPTextModel, CLIPTextModelOutput  # noqa: F401
 from .unet import AnimateDiffUNet3DModel, UNet3DConditionModel, UNet3DConditionOutput  # noqa: F401
 from .vae import AutoencoderKL, AutoencoderKLOutput, DecoderOutput, DiagonalGaussianDistribution  # noqa: F401
@@ -18,7 +19,7 @@ from .weights import seeded_state_dict  # noqa: F401
 
 # Name -> class lookup, mirroring videoswap/utils/registry.py (MODEL_REGISTRY / PIPELINE_REGISTRY) of the reference.
 MODEL_REGISTRY = {"AnimateDiffUNet3DModel": AnimateDiffUNet3DModel, "UNet3DConditionModel": AnimateDiffUNet3DModel,
-                  "SparsePointAdapter": SparsePointAdapter}
+                  "SparsePointAdapter": SparsePointAdapter, "T2IAdapter": T2IAdapter}
 PIPELINE_REGISTRY = {"VideoSwapPipeline": VideoSwapPipeline, "TuneAVideoPipeline": VideoSwapPipeline}
 
 

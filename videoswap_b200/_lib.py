@@ -130,6 +130,9 @@ _SIGNATURES = {
     "vs_downsample_conv3x3": (_I, [_P, _P, _I, _I, _I, _I, _P, _I, _P, _P]),
     "vs_vae_image_in": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "vs_vae_moments": (_I, [_P, _P, _I, _I, _I, _P, _P]),
+    "vs_t2i_image_in": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "vs_avgpool2x2": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "vs_scale_f16": (_I, [_P, _P, _SZ, _F, _P]),
     "vs_vae_posterior": (_I, [_P, _P, _P, _I, _I, _I, _F, _I, _P]),
     "vs_clip_embed": (_I, [_P, _P, _I, _I, _P, _I, _P, _I, _P]),
     "vs_causal_attention": (_I, [_P, _P, _I, _P, _I, _I, _I, _I, _I]),

@@ -10,7 +10,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvideoswap_b200.so")
-SOURCES = ["runtime.cu", "gemm.cu", "norm.cu", "attention.cu", "attention_tc.cu", "pointwise.cu", "unet.cu", "api.cu", "comm.cu", "text.cu", "dift.cu", "atlas.cu"]
+SOURCES = ["runtime.cu", "gemm.cu", "norm.cu", "attention.cu", "attention_tc.cu", "pointwise.cu", "unet.cu", "api.cu", "comm.cu", "text.cu", "dift.cu", "atlas.cu", "t2i_adapter.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "--use_fast_math" if False else "-DVS_NO_FAST_MATH"]

@@ -258,6 +258,15 @@ extern "C" int vs_downsample_conv3x3(void* stream, const void* d_x, int nimg, in
 extern "C" int vs_vae_image_in(void* stream, const void* d_x, int src_format, int nimg, int H, int W, void* d_out) {
   return vae_image_in((cudaStream_t)stream, d_x, src_format, nimg, H, W, (__half*)d_out);
 }
+extern "C" int vs_t2i_image_in(void* stream, const void* d_x, int nimg, int H, int W, int channels, void* d_out) {
+  return t2i_image_in((cudaStream_t)stream, (const uint8_t*)d_x, nimg, H, W, channels, (__half*)d_out);
+}
+extern "C" int vs_avgpool2x2(void* stream, const void* d_x, int nimg, int H, int W, int C, void* d_out) {
+  return avgpool2x2((cudaStream_t)stream, (const __half*)d_x, nimg, H, W, C, (__half*)d_out);
+}
+extern "C" int vs_scale_f16(void* stream, const void* d_x, size_t n, float scale, void* d_out) {
+  return scale_f16((cudaStream_t)stream, (const __half*)d_x, n, scale, (__half*)d_out);
+}
 extern "C" int vs_vae_moments(void* stream, const void* d_x, int nimg, int h, int w, const float* d_wb, void* d_out) {
   return vae_moments((cudaStream_t)stream, (const __half*)d_x, nimg, h, w, d_wb, (__half*)d_out);
 }

@@ -27,7 +27,7 @@
 // its taps through four parity views of the input (GemmParamsS2), so no im2col is materialised.
 //
 // Epilogue (per consumer warp, 16 rows of each 64-row half, one half after the other): registers -> [folded LayerNorm:
-// rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU / quick-GELU -> fp16 -> warp-private
+// rstd * acc - rstd * mean * u] + bias (+ time-embedding / positional row vector) / GEGLU / quick-GELU / ReLU -> fp16 -> warp-private
 // swizzled shared-memory transpose, 32 columns at a time -> (+ fp16 residual) -> coalesced 16-byte global stores.
 // Tiny-N or unaligned outputs (conv_out, N = 4) keep a direct-store path with the same rounding order.
 // The short-K linears (K <= 640, BN 128 / 160) and GEGLUs (K <= 640, BN 256; GemmParamsEpi) read no global memory in the
@@ -57,7 +57,7 @@ constexpr int EPI_COLS = 32;                        // output columns per epilog
 constexpr int EPI_WARP_BYTES = 16 * 64;             // per consumer warp: [16 rows x 64 B] transpose staging
 constexpr int EPI_BYTES = 8 * EPI_WARP_BYTES;
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
-enum { EPI_F_GEGLU = 1, EPI_F_RES = 2, EPI_F_RV = 4, EPI_F_LN = 8, EPI_F_LNOUT = 16, EPI_F_QGELU = 32 };   // compile-time epilogue features
+enum { EPI_F_GEGLU = 1, EPI_F_RES = 2, EPI_F_RV = 4, EPI_F_LN = 8, EPI_F_LNOUT = 16, EPI_F_QGELU = 32, EPI_F_RELU = 64 };   // compile-time epilogue features
 
 struct GemmParams {
   CUtensorMap tmA, tmA2, tmB;
@@ -172,6 +172,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   // pass that would re-read every such tensor from HBM.
   constexpr bool LNOUT = (EPI & EPI_F_LNOUT) != 0;
   constexpr bool QGELU = (EPI & EPI_F_QGELU) != 0;   // quick_gelu(acc + bias) (CLIP's MLP fc1)
+  constexpr bool RELU = (EPI & EPI_F_RELU) != 0;     // relu(acc + bias) (the T2I-Adapter's 3x3 block1 convs)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t epi_base = smem_base + C::STAGES * C::STAGE_BYTES;
@@ -523,6 +524,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
                 if constexpr (QGELU) {
                   f0 = quick_gelu_f(f0); f1 = quick_gelu_f(f1);
                 }
+                if constexpr (RELU) {
+                  f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
+                }
               }
               const __half2 hv = __floats2half2_rn(f0, f1);
               const uint32_t sa = stage_buf + sw64_off((lane >> 2) + 8 * h, jj) + 4 * q;
@@ -863,6 +867,10 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
     VS_REQUIRE(a.taps == 1 && p.staged && a.residual == nullptr && a.rowvec == nullptr && !a.ln_stats && !a.ln_parts &&
                a.ln_sums_out == nullptr && (bn == 128 || bn == 256),
                "gemm_tc: the quick-GELU epilogue takes a plain GEMM with a bias only, N %% 32 == 0 and BLOCK_N 128 / 256 (got %d)", bn);
+  if (a.mode == EPI_RELU)
+    VS_REQUIRE(a.taps == 9 && !two && !s2 && p.staged && a.residual == nullptr && a.rowvec == nullptr && !a.ln_stats &&
+               a.ln_sums_out == nullptr,
+               "gemm_tc: the ReLU epilogue takes a 3x3 conv of one source with a bias only and N %% 32 == 0");
   if (!p.staged) VS_REQUIRE(a.mode == EPI_LINEAR, "gemm_tc: GEGLU output needs 32-column aligned, 16-byte strided rows");
   if (a.ln_stats || a.ln_parts) VS_REQUIRE(p.staged && (reinterpret_cast<uintptr_t>(a.ln_u) & 15) == 0, "gemm_tc: folded LayerNorm needs the staged epilogue");
   if (a.ln_sums_out) VS_REQUIRE(p.staged, "gemm_tc: row statistics output needs the staged epilogue (N %% 32 == 0, aligned rows)");
@@ -873,6 +881,14 @@ int gemm_tc(cudaStream_t st, const GemmArgs& a) {
     return launch<256, EPI_F_GEGLU>(st, p);
   }
   if (a.mode == EPI_QUICK_GELU) return bn == 256 ? launch<256, EPI_F_QGELU>(st, p) : launch<128, EPI_F_QGELU>(st, p);
+  if (a.mode == EPI_RELU) {
+    switch (bn) {
+      case 64: return launch<64, EPI_F_RELU>(st, p);
+      case 128: return launch<128, EPI_F_RELU>(st, p);
+      case 256: return launch<256, EPI_F_RELU>(st, p);
+      default: return launch<160, EPI_F_RELU>(st, p);
+    }
+  }
   if (s2) {
     VS_REQUIRE(a.residual == nullptr && a.rowvec == nullptr && a.ln_sums_out == nullptr && p.staged,
                "gemm_tc: the stride-2 conv takes a bias only and needs N %% 32 == 0");

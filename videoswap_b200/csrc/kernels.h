@@ -7,7 +7,7 @@
 
 namespace vs {
 
-enum EpiMode { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_QUICK_GELU = 2 };
+enum EpiMode { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_QUICK_GELU = 2, EPI_RELU = 3 };
 
 // out[pix, n] = epilogue( sum_k A[pix(+tap shift), k] * Bw[n, k] )
 //   * plain GEMM (taps == 1): A is [M, K1] (lda1) optionally followed along K by A2 [M, K2] (channel concat).
@@ -15,7 +15,8 @@ enum EpiMode { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_QUICK_GELU = 2 };
 //     zero padding comes from TMA out-of-bounds fill.
 //   epilogue: + bias[n] + rowvec[pix / pix_per_batch, n] + residual[pix, n]; EPI_GEGLU: value*gelu(gate) on
 //   column-interleaved weights (see pack_geglu) -> N/2 output columns; EPI_QUICK_GELU: fp16((acc + bias) sigmoid(1.702
-//   (acc + bias))) (CLIP's quick_gelu; plain GEMM with a bias only, BLOCK_N 128 / 256).
+//   (acc + bias))) (CLIP's quick_gelu; plain GEMM with a bias only, BLOCK_N 128 / 256); EPI_RELU: fp16(max(acc + bias, 0))
+//   (3x3 conv of one source with a bias only, N % 32 == 0; the T2I-Adapter's resnet block1).
 struct GemmArgs {
   const __half* A = nullptr;  int K1 = 0;  int lda1 = 0;
   const __half* A2 = nullptr; int K2 = 0;  int lda2 = 0;
@@ -172,6 +173,14 @@ int cfg_ddim_rescale_step(cudaStream_t st, const void* eps2, const void* latents
 // Same, with (c_x, c_e, c_n, rescale) read from device memory.
 int cfg_ddim_rescale_step_dev(cudaStream_t st, const void* eps2, const void* latents, const void* noise, int is_f32, int S,
                               size_t n_s, int cfg, float guidance, const float* d_coef, void* out);
+// ---- T2I-Adapter (t2i_adapter.cu) --------------------------------------------------------------------------------
+// uint8 frames [nimg, H, W, c] (c = 1 or 3, H and W multiples of 8) -> the pixel-unshuffled fp16 NHWC input of conv_in,
+// [nimg, H / 8, W / 8, 64 c] with out[.., c' 64 + 8 i + j] = fp16(fp32(in[8 y + i, 8 x + j, c']) / 255).
+int t2i_image_in(cudaStream_t st, const uint8_t* x, int nimg, int H, int W, int c, __half* out);
+// 2x2 average pool, stride 2, NHWC fp16 [nimg, H, W, C] (H, W even, C % 8 == 0) -> [nimg, H / 2, W / 2, C], fp32 sum.
+int avgpool2x2(cudaStream_t st, const __half* x, int nimg, int H, int W, int C, __half* out);
+// out[i] = fp16(fp32(x[i]) * scale), n % 8 == 0; out may be x.
+int scale_f16(cudaStream_t st, const __half* x, size_t n, float scale, __half* out);
 // SparsePointAdapter splat: feat [P, C] fp32, tracks [F, P, 2] fp32 -> maps NHWC [F, h, w, C] fp16 (zeroed inside)
 int adapter_splat(cudaStream_t st, const float* feat, const float* tracks, const int* point_mask, int F, int P, int C,
                   int h, int w, float rate, int coord_fp16, float scale, __half* maps);

@@ -10,7 +10,7 @@ import torch
 from . import _lib
 
 GEGLU_GRANULE = 128
-EPI_LINEAR, EPI_GEGLU, EPI_QUICK_GELU = 0, 1, 2
+EPI_LINEAR, EPI_GEGLU, EPI_QUICK_GELU, EPI_RELU = 0, 1, 2, 3
 
 
 def set_option(name: str, value: int):
@@ -131,6 +131,49 @@ def conv3x3(x, w_packed, bias=None, x2=None, rowvec=None, imgs_per_batch=1, resi
     _gemm_ex(A=_ptr(x), K1=C1, lda1=C1, A2=_ptr(x2), K2=C2, lda2=C2, Bw=_ptr(w_packed), M=n * H * W, N=co, taps=9, nimg=n,
              H=H, W=W, bias=_ptr(bias), rowvec=_ptr(rowvec), ldrv=0 if rowvec is None else rowvec.stride(0),
              pix_per_batch=imgs_per_batch * H * W, residual=_ptr(residual), ldr=co, out=_ptr(out), ldc=co)
+    return out
+
+
+def conv3x3_relu(x, w_packed, bias=None, out=None):
+    """relu(conv3x3(x) + bias) in the conv's epilogue (one rounding to fp16): x [N, H, W, C] (C % 64 == 0), w_packed
+    [Co, 9 C] (Co % 32 == 0) -> [N, H, W, Co]."""
+    _chk16(x, w_packed)
+    _chk32(bias)
+    n, H, W, C1 = x.shape
+    co = w_packed.shape[0]
+    out = _out16(out, (n, H, W, co), x.device)
+    _gemm_ex(A=_ptr(x), K1=C1, lda1=C1, Bw=_ptr(w_packed), M=n * H * W, N=co, taps=9, nimg=n, H=H, W=W, bias=_ptr(bias),
+             out=_ptr(out), ldc=co, mode=EPI_RELU)
+    return out
+
+
+def t2i_image_in(frames):
+    """uint8 frames [n, H, W, c] (c = 1 or 3; H, W multiples of 8) -> F.pixel_unshuffle(frames / 255 as fp16, 8) in NHWC:
+    fp16 [n, H / 8, W / 8, 64 c], channel c' 64 + 8 i + j = pixel (8 y + i, 8 x + j) of channel c'."""
+    assert frames.is_cuda and frames.dtype == torch.uint8 and frames.is_contiguous() and frames.dim() == 4, \
+        "expected contiguous uint8 [n, H, W, c] CUDA frames"
+    assert frames.data_ptr() % 8 == 0, "frames must be 8-byte aligned"
+    n, H, W, c = frames.shape
+    out = torch.empty((n, H // 8, W // 8, 64 * c), dtype=torch.float16, device=frames.device)
+    _lib.call("vs_t2i_image_in", _stream(), _p(frames), n, H, W, c, _p(out))
+    return out
+
+
+def avgpool2x2(x):
+    """AvgPool2d(2, stride 2) of x [N, H, W, C] (H, W even, C % 8 == 0) -> [N, H / 2, W / 2, C], fp32 sum, one rounding."""
+    _chk16(x)
+    n, H, W, Cc = x.shape
+    out = torch.empty((n, H // 2, W // 2, Cc), dtype=torch.float16, device=x.device)
+    _lib.call("vs_avgpool2x2", _stream(), _p(x), n, H, W, Cc, _p(out))
+    return out
+
+
+def scale_f16(x, scale, out=None):
+    """fp16(fp32(x) * scale), as torch rounds an fp16 tensor times a Python float; out may be x (in place)."""
+    _chk16(x)
+    assert x.numel() % 8 == 0
+    out = _out16(out, tuple(x.shape), x.device)
+    _lib.call("vs_scale_f16", _stream(), _p(x), x.numel(), float(scale), _p(out))
     return out
 
 

@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import copy
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import nn
@@ -21,6 +21,7 @@ from .noise import randn_tensor
 from .formats import bind_concept_prompt
 from .scheduler import DDIMInverseScheduler, DDIMScheduler
 from .spec import adapter_param_shapes
+from .t2i_adapter import T2IAdapter
 from .unet import AnimateDiffUNet3DModel, _Holder
 from .vae import AutoencoderKL
 from .weights import seeded_state_dict
@@ -169,12 +170,17 @@ class VideoSwapPipeline:
     """The denoising loop of the reference pipeline on the native path.  BASELINE.json's `TuneAVideoPipeline` alias."""
 
     def __init__(self, unet: AnimateDiffUNet3DModel, scheduler: Optional[DDIMScheduler] = None,
-                 adapter: Optional[SparsePointAdapter] = None, inverse_scheduler: Optional[DDIMInverseScheduler] = None,
-                 vae: Optional[AutoencoderKL] = None, text_encoder=None, tokenizer=None):
-        """vae: encodes the source video for the inversion (invert(video=...)) and turns the final latents into frames
+                 adapter: Optional[Union[SparsePointAdapter, T2IAdapter]] = None,
+                 inverse_scheduler: Optional[DDIMInverseScheduler] = None, vae: Optional[AutoencoderKL] = None,
+                 text_encoder=None, tokenizer=None):
+        """adapter: a SparsePointAdapter (conditions: a TAP dict) or a T2IAdapter (conditions: a list of per-frame PIL
+        images); several adapters (diffusers' MultiAdapter) are not supported.
+        vae: encodes the source video for the inversion (invert(video=...)) and turns the final latents into frames
         (output_type "pt" / "np" / "pil"); without it the pipeline takes and returns latents only.
         text_encoder (text.CLIPTextModel) + tokenizer (transformers' CLIPTokenizer, or anything with its call interface):
         `prompt=` instead of `prompt_embeds` (encode_prompt)."""
+        if isinstance(adapter, (list, tuple)):
+            raise NotImplementedError("MultiAdapter (several adapters summed) is not implemented; give one adapter")
         self.unet = unet
         self.scheduler = scheduler or DDIMScheduler()
         self.inverse_scheduler = inverse_scheduler or DDIMInverseScheduler()
@@ -304,7 +310,11 @@ class VideoSwapPipeline:
         torch.Generator or a list of b.  eta > 0: DDIMScheduler.step's noise, drawn from `generator` at every step;
         guidance_rescale > 0: rescale_noise_cfg under CFG.  Mirrors pipeline_videoswap.py:552-610: output_type "latent"
         returns the latents [(b f), 4, h, w]; "pt" / "np" / "pil" decode them with the pipeline's vae (decode_latents).
-        `source_prompt` is accepted and unused; `num_images_per_prompt` must be 1."""
+        `source_prompt` is accepted and unused; `num_images_per_prompt` must be 1.
+        conditions: with a SparsePointAdapter the TAP dict (pred_tracks, img_size, point_embedding, index_list); with a
+        T2IAdapter one PIL image per frame (pipeline_videoswap.py:538-542, see t2i_adapter.preprocess_frames), whose
+        features are computed once per call.  Either way the residuals are scaled by t2i_guidance_scale, duplicated under
+        CFG and added at iterations i with len(timesteps) t2i_start <= i <= len(timesteps) t2i_end."""
         if num_images_per_prompt != 1:
             raise NotImplementedError("num_images_per_prompt must be 1 (one edited video per prompt)")
         if (prompt is None) == (prompt_embeds is None):
@@ -325,6 +335,20 @@ class VideoSwapPipeline:
             raise ValueError(f"{len(generator)} generators for a batch of {batch} videos")
         if latents is None and video_length is None:
             raise ValueError("drawing the latents from noise needs `video_length`")
+        cond_frames = None
+        if conditions is not None:
+            if self.adapter is None:
+                raise ValueError("conditions given but the pipeline has no adapter")
+            if isinstance(self.adapter, T2IAdapter):
+                if isinstance(conditions, dict):
+                    raise ValueError("a T2IAdapter takes a list of per-frame PIL images as conditions, not a TAP dict")
+                cond_frames = self.adapter.preprocess(conditions)           # checks only, no launch
+                frames = latents.shape[2] if latents is not None else video_length
+                if cond_frames.shape[0] != frames:
+                    raise ValueError(f"{cond_frames.shape[0]} condition images for {frames} frames")
+            elif not isinstance(conditions, dict):
+                raise ValueError("a SparsePointAdapter takes a TAP dict as conditions (pred_tracks, img_size, "
+                                 "point_embedding, index_list), not a list of images")
         if latents is not None and latents.shape[0] != batch:
             raise ValueError(f"latents hold {latents.shape[0]} videos, the prompts {batch}")
         if output_type != "latent":
@@ -347,9 +371,9 @@ class VideoSwapPipeline:
         if latents is None:
             latents = self.prepare_latents(batch, video_length, height, width, embeds.dtype, dev, generator)
         adapter_state = None
-        if conditions is not None:
-            if self.adapter is None:
-                raise ValueError("conditions given but the pipeline has no adapter")
+        if cond_frames is not None:
+            adapter_state = self._residuals_for_cfg(self.adapter(cond_frames, scale=t2i_guidance_scale), cfg)
+        elif conditions is not None:
             # the reference casts tracks AND the point embedding to the latents dtype first (pipeline_videoswap.py:528-533)
             emb = conditions["point_embedding"].to(dev)
             if latents.dtype == torch.float16:
